@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- encode_batch throughput of the B200 engine on BASELINE.json's headline config.
+"""bench.py -- encode_batch throughput of the CUDA engine (H100) on BASELINE.json's headline config.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--mb 1024] [--config gpt2|llama3|wordpiece]
+                    [--dump-outputs DIR]
 
 One step = one pass of the whole hot path (doc_mark -> pretok_scan -> page_scan -> long_find -> bpe_tile -> compaction)
 over one batch of the synthetic corpus of SURVEY.md 8(d) config 2 ("GPT-2 ByteLevel BPE, 1 GB synthetic UTF-8 docs avg
@@ -12,6 +13,10 @@ over one batch of the synthetic corpus of SURVEY.md 8(d) config 2 ("GPT-2 ByteLe
   roofline      the pre-tokenization scan kernel, CUDA events on its launch stream, against MEASURED_PEAKS.json
   configs       the other BASELINE configs (Llama-3 style, Whitespace + WordPiece, length-skew corpus) at 512 MB, fewer steps
   cpu_baseline  the reference's own Rust encode_batch (the `tokenizers` wheel) on this box's host cores, >= 256 MB sample
+
+--dump-outputs DIR (one GPU): after the timed steps, what the last device-resident step returned -- the ids and
+(char_start, char_end) offsets of a fixed, seeded sample of documents, with their indices and row lengths -- goes to
+DIR/<name>.npy in float32 / float64, so that two builds can be compared output for output on identical inputs.
 
 N > 1 (torchrun, one rank per GPU): every rank encodes its own byte-balanced shard of an N x 1 GB batch (weak scaling)
 through tokenizers_b200.parallel.encode_batch_sharded -- counts exchanged, every rank's compaction kernel writes at its
@@ -67,9 +72,9 @@ def gen_corpus(kind, seed, first_doc, n_docs, max_bytes, out):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit,name")
 
     def __init__(self, gpus):
         self.gpus, self.p, self.lines = list(gpus), None, []
@@ -95,11 +100,12 @@ class ClockSampler:
             self.p.wait(timeout=2)
         except Exception:
             self.p.kill()
-        sm, mx, reasons = {}, [], set()
+        sm, mx, reasons, cards = {}, [], set(), set()
         for ln in self.lines:
             f = [x.strip() for x in ln.split(",")]
-            if len(f) < 8:
+            if len(f) < 10:
                 continue
+            cards.add((f[9], f[8]))
             try:
                 sm.setdefault(f[0], []).append(float(f[1])); mx.append(float(f[2]))
             except ValueError:
@@ -110,7 +116,8 @@ class ClockSampler:
         med = {g: float(np.median(v)) for g, v in sorted(sm.items(), key=lambda kv: (len(kv[0]), kv[0]))}
         # sm_mhz: the slowest GPU's median under load (every rank's GPU is sampled, not only rank 0's)
         return {"sm_mhz": min(med.values()) if med else None, "sm_max_mhz": max(mx) if mx else None, "reasons": sorted(reasons),
-                "samples": min((len(v) for v in sm.values()), default=0), "per_gpu_sm_mhz": list(med.values())}
+                "samples": min((len(v) for v in sm.values()), default=0), "per_gpu_sm_mhz": list(med.values()),
+                "gpus": [{"name": nm, "power_limit_w": pl} for nm, pl in sorted(cards)]}
 
 
 def cpu_reference_worker(cfg, threads, budget_s, min_mb):
@@ -197,8 +204,34 @@ class DevArr:  # zero-copy torch view of an engine-owned device buffer
         self.__cuda_array_interface__ = {"shape": (count,), "typestr": typestr, "data": (ptr, False), "version": 3}
 
 
-def measure(ctx, cfg, kind, mb, steps, warmup, sharded=False, special=None):
-    """Device-resident and end-to-end numbers of one configuration on this rank.  Returns a dict of raw measurements."""
+DUMP_DOCS, DUMP_BYTES = 16384, 64 << 20
+
+
+def dump_outputs(out_dir, L, res, n_docs):
+    """Writes the CSR of a device-resident result (ids + char offsets) for a seeded sample of its documents: the whole
+    CSR of a 1 GB batch is ~3 GB, the sample stays under DUMP_BYTES.  Ids, offsets and row lengths are below 2^24, so
+    float32 holds them exactly; document indices are float64."""
+    import torch
+    T = int(L.b2t_result_n_tokens(res))
+    rp = torch.as_tensor(DevArr(L.b2t_result_row_ptr(res), n_docs + 1, "<i8"), device="cuda").cpu().numpy()
+    docs = np.sort(np.random.default_rng(0).choice(n_docs, size=min(n_docs, DUMP_DOCS), replace=False))
+    lens = rp[docs + 1] - rp[docs]
+    keep = int(np.searchsorted(np.cumsum(lens * 12 + 16), DUMP_BYTES - (1 << 20), side="right"))  # 4 B id + 8 B offsets per token
+    docs, lens = docs[:keep], lens[:keep]
+    tok = torch.from_numpy(np.repeat(rp[docs], lens) + np.arange(int(lens.sum())) - np.repeat(np.cumsum(lens) - lens, lens)).cuda()
+    ids = torch.as_tensor(DevArr(L.b2t_result_ids(res), T, "<i4"), device="cuda")[tok]
+    offs = torch.as_tensor(DevArr(L.b2t_result_offsets(res), 2 * T, "<i4"), device="cuda").view(T, 2)[tok]
+    os.makedirs(out_dir, exist_ok=True)
+    for name, arr in (("doc_index", docs.astype(np.float64)), ("row_lengths", lens.astype(np.float32)),
+                      ("ids", ids.cpu().numpy().view(np.uint32).astype(np.float32)),
+                      ("offsets", offs.cpu().numpy().view(np.uint32).astype(np.float32)),
+                      ("totals", np.array([n_docs, T], dtype=np.float64))):
+        np.save(os.path.join(out_dir, name + ".npy"), arr)
+
+
+def measure(ctx, cfg, kind, mb, steps, warmup, sharded=False, special=None, dump_dir=None):
+    """Device-resident and end-to-end numbers of one configuration on this rank.  Returns a dict of raw measurements.
+    dump_dir: where the last device-resident step's output goes (dump_outputs)."""
     import torch
     from tokenizers_b200 import Tokenizer, _lib
     L, rank, world, local = ctx["L"], ctx["rank"], ctx["world"], ctx["local"]
@@ -229,9 +262,7 @@ def measure(ctx, cfg, kind, mb, steps, warmup, sharded=False, special=None):
     def step_device():
         res = ctypes.c_void_p()
         _lib.check(L.b2t_encode_batch_device(tok.handle, d_bytes.data_ptr(), n, d_off.data_ptr(), n_docs, flags, ctypes.c_void_p(stream.cuda_stream), ctypes.byref(res)))
-        T = L.b2t_result_n_tokens(res)
-        L.b2t_result_free(res)
-        return T
+        return L.b2t_result_n_tokens(res), res
 
     def barrier():
         torch.cuda.synchronize()
@@ -240,13 +271,16 @@ def measure(ctx, cfg, kind, mb, steps, warmup, sharded=False, special=None):
 
     names = (ctypes.c_char_p * 16)(); ms = (ctypes.c_float * 16)()
     for _ in range(warmup):
-        T = step_device()
+        T, res = step_device()
+        L.b2t_result_free(res)
     barrier()
     kern_ms, launches = {}, 0
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record(stream)
-    for _ in range(steps):
-        T = step_device()
+    for i in range(steps):
+        if i:
+            L.b2t_result_free(res)   # the last step's result stays alive for dump_outputs
+        T, res = step_device()
         launches += L.b2t_engine_last_kernels(tok.handle, names, ms, 16)
         for i in range(16):
             if names[i] is None:
@@ -258,6 +292,9 @@ def measure(ctx, cfg, kind, mb, steps, warmup, sharded=False, special=None):
     barrier()
     dev_ms = ev0.elapsed_time(ev1)
     _lib.check(L.b2t_engine_set_profiling(tok.handle, 0))
+    if dump_dir is not None:
+        dump_outputs(dump_dir, L, res, n_docs)
+    L.b2t_result_free(res)
 
     # ---- N > 1: the sharded product path, exchange of step i overlapping the kernels of step i + 1
     shard_ms = None
@@ -359,21 +396,13 @@ def measure_api(ctx, cfg, mb=128):
 
 
 def roofline_of(m, peaks, cfg):
-    peak = peaks.get("hbm_gbs", 6650.0)
+    peak = peaks.get("hbm_gbs", 3350.0)
     k1 = m["kern_ms"].get("pretok_scan", float("nan"))
     n = m["n"]
     k1_bytes = n * 1.25 + (n / 2048) * 8  # bytes + doc_bits in, start_bits + page summaries out (DESIGN.md)
-    traffic, src = None, None
-    try:  # dram bytes of one launch from the committed ncu --set full capture (profiles/), scaled by input size
-        tj = json.load(open(os.path.join(ROOT, "profiles", "k1_traffic.json")))
-        if tj.get("config") == cfg:
-            traffic, src = tj["dram_bytes_per_input_byte"] * n, tj.get("source", "profiles/k1_traffic.json")
-    except Exception:
-        pass
     return {"kernel": "pretok_lean_kernel" if cfg != "llama3" else "pretok_stream_kernel", "bound": "hbm", "achieved": k1_bytes / (k1 * 1e-3) / 1e9, "peak": peak,
-            "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if "hbm_gbs" in peaks else "B200_PROFILING.md fallback (of fallback)",
-            "unit": "GB/s", "frac": k1_bytes / (k1 * 1e-3) / 1e9 / peak, "traffic": traffic,
-            "traffic_source": (f"ncu capture {src}, dram bytes per input byte x this launch's input bytes (not re-measured in this run)" if traffic else None),
+            "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3.35 TB/s",
+            "unit": "GB/s", "frac": k1_bytes / (k1 * 1e-3) / 1e9 / peak,
             "algorithmic_bytes_per_launch": k1_bytes, "ms_per_launch": k1, "input_GBps": n / (k1 * 1e-3) / 1e9,
             "frac_survey_8d_accounting": (n * 1.75) / (k1 * 1e-3) / 1e9 / peak,
             "note": "achieved uses THIS kernel's layout (bytes + doc bitmap in, split bitmap + page summaries out = 1.25 B per input byte); "
@@ -397,7 +426,12 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-configs", action="store_true", help="skip the secondary configs (llama3 / wordpiece / skew)")
     ap.add_argument("--kind", type=int, default=0, help="corpus kind override (5 = length-skew stress of BASELINE configs[4])")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's output (a seeded sample) as DIR/<name>.npy")
     a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
+    if a.dump_outputs and a.impl == "reference":
+        ap.error("--dump-outputs writes the GPU path's output; --impl reference has none")
     a.warmup = max(a.warmup, 3) if a.impl != "reference" else a.warmup
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local = int(os.environ.get("LOCAL_RANK", "0"))
     cfg = a.config
@@ -441,7 +475,9 @@ def main():
     if rank == 0:
         sampler.start()  # samples every 50 ms from the warm-up through the timed device and e2e regions
     kind = a.kind or KIND[cfg]
-    m = measure(ctx, cfg, kind, a.mb, a.steps, a.warmup, sharded=True)
+    if a.dump_outputs and world > 1:
+        ap.error("--dump-outputs takes one GPU")
+    m = measure(ctx, cfg, kind, a.mb, a.steps, a.warmup, sharded=True, dump_dir=a.dump_outputs)
     clocks = sampler.stop() if rank == 0 else None
 
     # ---- reduce over ranks: time = max, work = sum

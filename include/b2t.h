@@ -1,14 +1,14 @@
-/* b2t.h -- C ABI of the B200 batched tokenization engine (libb2t.so).
+/* b2t.h -- C ABI of the CUDA (H100, sm_90a) batched tokenization engine (libb2t.so).
  *
  * Drop-in boundary for ONE path of huggingface/tokenizers: `Tokenizer::encode_batch` for ByteLevel-BPE
  * (GPT-2 / Llama-3 style) and Whitespace + WordPiece.  Each entry point names the reference interface it
- * replaces (paths relative to /root/reference/tokenizers/src unless noted).  A Rust host would bind this file
+ * replaces (paths relative to tokenizers/src of huggingface/tokenizers unless noted).  A Rust host would bind this file
  * with an `extern "C"` block (see INTEGRATION.md); the Python shim in tokenizers_b200/ binds it with ctypes.
  *
  * Conventions: plain pointers and sizes only; every function returns a b2t_status value (0 = ok) unless noted; the
  * message of the last error on the calling thread is available from b2t_last_error().  No CPU fallback exists:
  * configurations outside the supported set fail with B2T_ERR_UNSUPPORTED, and every encode entry point needs a
- * CUDA device (sm_100a).
+ * CUDA device (sm_90a).
  */
 #ifndef B2T_H_
 #define B2T_H_

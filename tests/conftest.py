@@ -6,4 +6,4 @@ for p in (ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tools")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Generate tests/golden/golden_*.json.gz by running the REFERENCE implementation (the `tokenizers` wheel, same Rust core
-as /root/reference) on seeded inputs.  Run in the dev container; the outputs are committed and are what pins the
+as huggingface/tokenizers) on seeded inputs.  The outputs are committed and are what pins the
 oracle (and, through it, the CUDA path) on boxes where the wheel is not consulted.
 
 Each file: {"tokenizer": <tokenizer.json dict or asset name>, "cases": [{"input", "ids", "offsets", "word_ids"}...]}

@@ -89,6 +89,20 @@ def wheel_csr(tok, docs):
     return cases_to_csr([{"ids": e.ids, "offsets": e.offsets, "word_ids": e.word_ids} for e in encs])
 
 
+# corpus.generate arguments of the large comparison with the reference wheel (golden/wheel_large_digests.json)
+WHEEL_LARGE_CORPUS = {"gpt2_style": (2, 99, 0, 40000), "llama3_style": (2, 99, 0, 40000), "wordpiece": (4, 99, 0, 40000)}
+
+
+def csr_digests(csr):
+    """SHA-256 of each CSR array (ids u32, offsets u32 [T, 2], word ids u32, row_ptr u64) and the token count"""
+    import hashlib
+    dts = (np.uint32, np.uint32, np.uint32, np.uint64)
+    d = {nm: hashlib.sha256(np.ascontiguousarray(np.asarray(a).reshape(-1), dtype=dt).tobytes()).hexdigest()
+         for nm, a, dt in zip(("ids", "offsets", "word_ids", "row_ptr"), csr, dts)}
+    d["n_tokens"] = int(np.asarray(csr[0]).size)
+    return d
+
+
 # ---------------------------------------------------------------------------------------------- host-logic harness
 def oracle_backed_tokenizer(tokenizer_json):
     """TEST ONLY: tokenizers_b200.Tokenizer's host logic (added tokens, templates, CSR stitching) in front of the ORACLE

@@ -1,4 +1,4 @@
-"""tokenizers_b200 -- B200-native batched tokenization engine behind the `Tokenizer.encode_batch` surface of
+"""tokenizers_b200 -- CUDA (H100) batched tokenization engine behind the `Tokenizer.encode_batch` surface of
 huggingface/tokenizers (ByteLevel-BPE and Whitespace+WordPiece).  See DESIGN.md / INTEGRATION.md."""
 from .tokenizer import Tokenizer, Encoding, BatchEncoding, UnsupportedConfig, parse_tokenizer_json  # noqa: F401
 from ._lib import B2TError  # noqa: F401

@@ -1,6 +1,6 @@
 // added_kernels.cuh -- added / special token extraction on the device, in front of the pre-tokenization scan.
 //
-// Replaces, for pipelines without a normalizer (paths relative to /root/reference/tokenizers/src):
+// Replaces, for pipelines without a normalizer (paths relative to tokenizers/src of huggingface/tokenizers):
 //   tokenizer/added_vocabulary.rs:523-564  extract_and_normalize: the text is split on the added tokens with
 //                                          normalized == false first, then every remaining piece on the normalized ones
 //   tokenizer/added_vocabulary.rs:430-490  find_matches: leftmost-longest, non-overlapping matches (the reference builds an

@@ -1,7 +1,7 @@
 // dense_kernels.cuh -- the post-path steps of a single-sequence batch on the device: special-token template, truncation
 // and padding, emitted as dense [n_docs, L] id / attention-mask tensors straight from the token CSR.
 //
-// Replaces, for batches of single sequences (paths relative to /root/reference/tokenizers/src):
+// Replaces, for batches of single sequences (paths relative to tokenizers/src of huggingface/tokenizers):
 //   tokenizer/mod.rs:1265-1317       TokenizerImpl::post_process: truncate to max_length - n_added_tokens, template, padding
 //   utils/truncation.rs:70-166       truncate_encodings, single sequence: keep the first (direction right) or the last
 //                                    (direction left) max_length tokens -- the kept part of Encoding::truncate

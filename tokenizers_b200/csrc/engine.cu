@@ -47,7 +47,7 @@ static int fail(int code, const char* fmt, ...) {
   } while (0)
 
 extern "C" const char* b2t_last_error(void) { return g_err; }
-extern "C" const char* b2t_version(void) { return "tokenizers_b200 0.1 (sm_100a)"; }
+extern "C" const char* b2t_version(void) { return "tokenizers_b200 0.1 (sm_90a)"; }
 
 #ifdef B2T_K1_DEBUG
 extern "C" int b2t_debug_k1(uint32_t* out, size_t words) {
@@ -178,7 +178,7 @@ constexpr int MAX_KERNEL_RECORDS = 16;
 struct b2t_engine {
   int device = 0;
   int model = 0, pretok = 0, add_prefix_space = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   int wcache_on = 1;         // B2T_WCACHE=0: no word cache, every pre-token is merged (the reference benches cache_capacity(0) too)
   int k1_tiled = 0;          // B2T_K1_TILED=1: the round-1 shared-memory-tiled scan (kept for A/B runs)
   DeviceTables dt;
@@ -529,7 +529,8 @@ static int run_device_pipeline(b2t_engine* e, Workspace& ws, const uint8_t* d_by
     return rc;
   if (pretok_drops_whitespace(e->pretok) && (rc = ws.drop_bits.ensure(n_words * 4))) return rc;
   const bool bpe = e->model == B2T_MODEL_BPE;
-  // measured on the 1 GB corpus: 2^19 slots 19.5 ms, 2^20 17.0, 2^21 16.3, 2^22 15.8 (bpe_tile); 2^21 x 64 B = 128 MiB
+  // bpe_tile on the 1 GB corpus, H100 80GB HBM3 at a 400 W power limit: 2^19 slots 19.7 ms, 2^20 18.6, 2^21 17.4-17.5,
+  // 2^22 17.1; 2^21 x 64 B = 128 MiB
   constexpr uint32_t WCACHE_SLOTS = 1u << 21;
   if (model_pass && (rc = ws.wcache.ensure((size_t)WCACHE_SLOTS * 64))) return rc;
   if (model_pass && bpe) {

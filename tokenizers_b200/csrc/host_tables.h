@@ -1,6 +1,6 @@
 // host_tables.h -- host-side construction of the device tables from the engine configuration.
 //
-// Restates the one-time table building of the reference (paths relative to /root/reference/tokenizers/src):
+// Restates the one-time table building of the reference (paths relative to tokenizers/src of huggingface/tokenizers):
 //   pre_tokenizers/byte_level.rs:15-39   bytes_char(): the byte <-> unicode char map of ByteLevel
 //   models/bpe/model.rs:252-275          merges (a, b) -> ids through the vocab, new token = a + b
 //   models/wordpiece/mod.rs:143-153      vocab, unk token, continuing subword prefix

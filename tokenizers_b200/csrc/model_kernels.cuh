@@ -1,6 +1,6 @@
 // model_kernels.cuh -- K2: one tile kernel that turns (bytes, pre-token bitmap) into the token CSR.
 //
-// Replaces, per 2 KB page of the packed batch (paths relative to /root/reference/tokenizers/src):
+// Replaces, per 2 KB page of the packed batch (paths relative to tokenizers/src of huggingface/tokenizers):
 //   models/bpe/model.rs:465-612 (merge_word, tokenize_with_cache incl. ignore_merges) + models/bpe/word.rs:162-268
 //   models/wordpiece/mod.rs:224-283 (greedy longest match, max_input_chars_per_word, [UNK])
 //   tokenizer/pre_tokenizer.rs:198-263,329-364 (into_encoding: offsets -> original -> char, word ids)
@@ -113,9 +113,8 @@ __device__ __forceinline__ uint32_t tok_id(uint32_t x) { return x & ((1u << TOK_
 constexpr int WC_MAX_BYTES = 24, WC_MAX_TOK = 6, WC_PROBES = 4;
 // Cache misses of up to P4_SPLIT_BYTES bytes are merged by 8 lanes x 2 positions, longer ones (<= THREAD_PATH_MAX) by
 // 8 lanes x 4, in separate passes: the groups of a warp step through their merge rounds together, so a warp should
-// hold words of similar length.  Measured on B200 (512 MB, bpe_tile): one mixed pass 8.15 ms, split at 12: 8.07 (one
-// loop) / 8.62 (two passes), split at 16 in two passes 7.95; 4 or 2 lanes per short word 9.0 / 12.8 ms (more words per
-// warp = more rounds per pass: the rounds are L2-latency bound, not lane bound).
+// hold words of similar length.  Fewer lanes per short word mean more words per warp and so more rounds per pass: the
+// rounds are L2-latency bound, not lane bound.
 constexpr int P4_SPLIT_BYTES = 16;
 constexpr int P4_SHORT_G = 8;
 template <int V> struct IntTag { static constexpr int value = V; };
@@ -332,7 +331,7 @@ __device__ __forceinline__ void coop_bpe(const DeviceTables& t, const uint8_t* s
 
 
 #ifndef B2T_MINBLOCKS
-#define B2T_MINBLOCKS 8  // measured on B200: 8 blocks/SM (32 regs, small spills) beats 5 (48 regs) by 15 %: the kernel is latency-bound
+#define B2T_MINBLOCKS 8  // 8 blocks/SM (32 regs, small spills) rather than 5 (48 regs): the kernel is latency-bound
 #endif
 template <int MODEL>
 __global__ void __launch_bounds__(MODEL_THREADS, B2T_MINBLOCKS) model_tile_kernel(const ModelParams P) {
@@ -581,7 +580,7 @@ __global__ void __launch_bounds__(MODEL_THREADS, B2T_MINBLOCKS) model_tile_kerne
       }
       // warp-aggregated queue appends
       // the four groups of a warp step through their merges together, so pre-tokens of similar length should share a
-      // warp: short misses queue from the front of s_miss, longer ones from the back (measured: -1.5 % kernel time)
+      // warp: short misses queue from the front of s_miss, longer ones from the back
       const bool longer = kind == 1 && (int)s_pt[k + 1] - (int)s_pt[k] > P4_SPLIT_BYTES;
       const unsigned mm = __ballot_sync(0xFFFFFFFFu, kind == 1 && !longer), mh = __ballot_sync(0xFFFFFFFFu, longer),
                      mq = __ballot_sync(0xFFFFFFFFu, kind == 2);
@@ -618,7 +617,7 @@ __global__ void __launch_bounds__(MODEL_THREADS, B2T_MINBLOCKS) model_tile_kerne
           }
           coop_bpe<G, J>(P.t, s_byte, s_tok, s, e, active, gl);
           __syncwarp();
-          // long numbers rarely repeat: publishing them only fills the table (measured: -5 % kernel time without them)
+          // long numbers rarely repeat: publishing them only fills the table
           const bool numeric = active0 && (e - s) >= 5 && (unsigned)(s_byte[s + 1] - '0') < 10u && (unsigned)(s_byte[e - 1] - '0') < 10u;
           if (P.wcache_on && active0 && gl == 0 && e - s <= WC_MAX_BYTES && !numeric && !(P.t.ignore_merges && is_piece(s, e))) {
             WordKey key;
@@ -630,9 +629,8 @@ __global__ void __launch_bounds__(MODEL_THREADS, B2T_MINBLOCKS) model_tile_kerne
       // longer pre-tokens (17..32 bytes: rare, many rounds) by lane groups
       run_misses(IntTag<8>{}, IntTag<THREAD_PATH_MAX / 8>{}, n_longer, true);
       // short ones (<= 16 bytes: nearly all misses) with fewer positions per lane.  (One THREAD per short miss, 32 words per
-      // warp with the pair ranks in shared memory, needs 4-5x fewer instructions per word but was measured SLOWER, with the
-      // cache on (+5 %) and off (+39 %): the page waits for its longest chain of dependent probes, and a lane group's chain
-      // is the shortest -- profiles/k2_experiments_r02.md.)
+      // warp with the pair ranks in shared memory, needs 4-5x fewer instructions per word but was slower when tried, with the
+      // cache on and off: the page waits for its longest chain of dependent probes, and a lane group's chain is the shortest.)
       run_misses(IntTag<P4_SHORT_G>{}, IntTag<(P4_SPLIT_BYTES + P4_SHORT_G - 1) / P4_SHORT_G>{}, n_short, false);
     }
     // -------------------------------------------------------------- P4b: one warp per longer pre-token (33..256 bytes)
@@ -753,7 +751,7 @@ __global__ void __launch_bounds__(MODEL_THREADS, B2T_MINBLOCKS) model_tile_kerne
       if ((tb >> lane) & 1u) s_tokpos[s_tpref[row] + __popc(tb & ((1u << lane) - 1u))] = (uint16_t)(row * 32 + lane);
     }
     // ---------------------------------------------------------------- P6: page token count (no ordering between pages:
-    // an in-order look-back chain stalled every page behind the slowest of ~1000 pages in flight -- profiles/)
+    // an in-order look-back chain stalls every page behind the slowest of the pages in flight)
     if (tid == 0) {
       const int A = s_ntok + ((MODEL == MODEL_WORDPIECE && long_kept) ? 1 : 0) + (MODEL == MODEL_BPE ? s_lcum[n_longs] : 0);
       s_ntot = A;

@@ -1,6 +1,6 @@
 // norm_kernels.cuh -- BertNormalizer on the device, as a byte-rewriting pre-pass in front of the scan kernels.
 //
-// Replaces (paths relative to /root/reference/tokenizers/src):
+// Replaces (paths relative to tokenizers/src of huggingface/tokenizers):
 //   normalizers/bert.rs:92-136          clean_text, handle_chinese_chars, strip_accents (NFD + drop Mn), lowercase
 //   tokenizer/normalizer.rs:317-428     NormalizedString::transform: the alignment of every normalized character with
 //                                       the original character it came from, which is what token offsets are made of

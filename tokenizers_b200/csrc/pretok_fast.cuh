@@ -36,7 +36,7 @@ B2T_HD uint32_t fsl(uint32_t lo, uint32_t hi, int k) { return (uint32_t)(((((uin
 B2T_HD uint32_t fsr(uint32_t lo, uint32_t hi, int k) { return (uint32_t)((((uint64_t)hi << 32) | lo) >> k); }
 #endif
 // x >> K for a constant K.  On the device as a multiply-high: the shift units share the integer pipe with the logic
-// ops that bound this kernel, the multiplier sits on the other pipe (measured on B200: no gain, the multiply-high is no cheaper than the shift -- kept switchable, off by default).
+// ops that bound this kernel, the multiplier sits on the other pipe (kept switchable, off by default).
 #ifndef B2T_SHR_MULHI
 #define B2T_SHR_MULHI 0
 #endif
@@ -49,8 +49,8 @@ B2T_HD uint32_t shr(uint32_t x) {
 #endif
 }
 // 3-input look-up: bit (a b c) of TB.  Written as a sum of minterms over three variables, which nvcc folds into ONE LOP3.
-// (An inline-asm lop3 here produced wrong class masks on sm_100a when the call sat next to a warp vote -- measured on
-// the GPU against the CPU run of this very file, profiles/k1_experiments_r02.md -- so the compiler does the folding.)
+// (An inline-asm lop3 here once produced wrong class masks when the call sat next to a warp vote -- seen on the GPU
+// against the CPU run of this very file -- so the compiler does the folding.)
 template <uint32_t TB>
 B2T_HD uint32_t lop3(uint32_t a, uint32_t b, uint32_t c) {
   uint32_t d = 0;

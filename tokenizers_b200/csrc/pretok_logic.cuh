@@ -94,7 +94,7 @@ B2T_HD uint32_t decode_at(const ByteAt& at, int64_t p, int64_t end, int* len) {
 // Outputs: m.L / m.N / m.S / m.SP / m.NL / m.AP for ASCII bytes only, *hi = non-ASCII bytes, *cont = continuation bytes.
 // kind: PT_WHITESPACE uses the Rust-regex classes (\w on ASCII = [0-9A-Za-z_], N slot unused).
 // `one` must be 1 at run time and opaque to the compiler: x * one + c makes the SWAR adds IMADs (FMA pipe) instead of
-// IADD3s, so they no longer compete with the LOP3 / SHF work for the ALU pipe (each pipe issues 1 warp-instr / 2 clk).
+// IADD3s, so they no longer compete with the LOP3 / SHF work for the ALU pipe.
 B2T_HD void ascii_masks(int kind, const uint32_t w[8], ChunkMasks& m, uint32_t* hi_out, uint32_t* cont_out, uint32_t one = 1u) {
   const bool rust = kind == PT_WHITESPACE;
   uint32_t L = 0, N = 0, SP = 0, CT = 0, HI = 0, any_ctl = 0, any_ap = 0, any_hi = 0;

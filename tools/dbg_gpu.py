@@ -1,5 +1,5 @@
 import sys, os, ctypes, numpy as np
-ROOT=os.environ.get("GRAFT_REPO_ROOT","/root/repo")
+ROOT=os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0,ROOT); sys.path.insert(0,ROOT+"/tests"); sys.path.insert(0,ROOT+"/tools")
 import helpers, fuzzgen
 from tokenizers_b200 import Tokenizer, _lib

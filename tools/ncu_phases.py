@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Sum ncu per-SASS-instruction counts and stall samples of the page kernel by phase (source-line ranges of
 model_kernels.cuh).  Usage: ncu_phases.py <src.csv> <kernel substring> <sass file>"""
-import csv, re, sys
+import csv, os, re, sys
 src_csv, kname, sass = sys.argv[1], sys.argv[2], sys.argv[3]
 rows = list(csv.reader(open(src_csv)))
 h = rows[1]; ix = h.index("Instructions Executed"); ns = h.index("# Samples"); tx = h.index("Thread Instructions Executed")
@@ -18,7 +18,7 @@ for ln in lines:
     m = re.search(r'//## File "([^"]+)", line (\d+)', ln)
     if m: cur = (m.group(1).split("/")[-1], int(m.group(2))); continue
     if re.match(r"\s+/\*[0-9a-f]{4,}\*/", ln): locs.append(cur)
-src = open("/root/repo/tokenizers_b200/csrc/model_kernels.cuh").read().split("\n")
+src = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tokenizers_b200", "csrc", "model_kernels.cuh")).read().split("\n")
 # phase markers: a phase starts at the first line containing the marker text
 marks = [("wc_make_key", "__device__ __forceinline__ void wc_make_key"), ("wc_lookup", "__device__ __forceinline__ bool wc_lookup"),
          ("wc_publish", "__device__ __forceinline__ void wc_publish"), ("vocab_whole", "__device__ __forceinline__ bool vocab_whole_word"),

@@ -1,5 +1,5 @@
 // Micro-benchmark: issue rates of the integer instructions the scan kernel is made of, alone and mixed (developer tool).
-// nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o pipes pipes.cu && ./pipes
+// nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o pipes pipes.cu && ./pipes
 #include <cstdio>
 #include <cuda_runtime.h>
 #define ITERS 4096
@@ -28,17 +28,17 @@ __global__ void k(unsigned* out, unsigned m1, unsigned m2, unsigned sh) {
 }
 template <int MODE>
 void run(const char* name, int ops) {
-  unsigned* out; cudaMalloc(&out, 148 * 8 * 256 * 4);
+  int sms, khz; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0); cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
+  unsigned* out; cudaMalloc(&out, sms * 8 * 256 * 4);
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-  k<MODE><<<148 * 8, 256>>>(out, 0x55555555u, 0x33333333u, 4u);
+  k<MODE><<<sms * 8, 256>>>(out, 0x55555555u, 0x33333333u, 4u);
   cudaEventRecord(e0);
-  k<MODE><<<148 * 8, 256>>>(out, 0x55555555u, 0x33333333u, 4u);
+  k<MODE><<<sms * 8, 256>>>(out, 0x55555555u, 0x33333333u, 4u);
   cudaEventRecord(e1); cudaEventSynchronize(e1);
   float ms; cudaEventElapsedTime(&ms, e0, e1);
-  int mhz; cudaDeviceGetAttribute(&mhz, cudaDevAttrClockRate, 0);
-  double warp_instr = 148.0 * 8 * 8 * ITERS * 4 * ops;      // per kernel
-  double cyc = ms * 1e-3 * 1.965e9;
-  printf("%-28s %7.3f ms  %6.2f warp-instr/clk/SM (of the %d counted ops per group)\n", name, ms, warp_instr / cyc / 148.0, ops);
+  double warp_instr = (double)sms * 8 * 8 * ITERS * 4 * ops;      // per kernel
+  double cyc = ms * 1e-3 * khz * 1e3;                              // at the maximum SM clock the device reports
+  printf("%-28s %7.3f ms  %6.2f warp-instr/clk/SM (of the %d counted ops per group)\n", name, ms, warp_instr / cyc / sms, ops);
   cudaFree(out);
 }
 int main() {
