@@ -54,11 +54,11 @@ extern "C" int b2t_emul_pretok(int kind, const uint8_t* bytes, uint64_t n, const
 
 // The streaming kernel's composition, chunk by chunk: classification (bit planes, certain classes, table look-ups, fill,
 // spill-in from the previous chunk), the 32-bit boundary algebra with the next chunk's first-byte bits, contraction
-// overflow into the next chunk, and the exact window code for chunks that ask for the fallback.
-// fallbacks_out (optional): number of chunks that took the fallback.
+// overflow into the next chunk, and finalize_gpt2 with the next chunk's first bits.
+// fallbacks_out (optional): number of chunks whose straddling multi-byte space finalize_gpt2 gave back.
 template <int KIND>
 static void emul_fast(const uint8_t* bytes, uint64_t n, const uint64_t* doc_off, uint32_t n_docs, const uint32_t* cls_tbl,
-                      uint32_t* start_bits, uint32_t* drop_bits, uint64_t* fallbacks_out, uint32_t* planes_out = nullptr) {
+                      uint32_t* start_bits, uint32_t* drop_bits, uint64_t* fallbacks_out) {
   const int64_t n_chunks = (int64_t)(n / CHUNK) + 1;
   std::vector<uint32_t> DS(n_chunks + 2, 0);
   for (uint32_t d = 0; d <= n_docs; ++d) DS[doc_off[d] / 32] |= 1u << (doc_off[d] % 32);
@@ -85,27 +85,6 @@ static void emul_fast(const uint8_t* bytes, uint64_t n, const uint64_t* doc_off,
     if (m.cont & 1u) spill_in(m, pt.L, pt.N, pt.S);
     M[c] = m; PT[c] = pt; prev = m;
   }
-  // exact window code (pretok_logic.cuh) for the fallback
-  auto exact = [&](int64_t c, uint32_t* drop) -> uint32_t {
-    auto masks = [&](int64_t k) -> ChunkMasks {
-      ChunkMasks z; std::memset(&z, 0, sizeof(z));
-      if (k < 0 || k >= n_chunks) return z;
-      uint32_t w[8];
-      for (int j = 0; j < 8; ++j) { uint32_t x = 0; for (int q = 0; q < 4; ++q) x |= at(k * 32 + j * 4 + q) << (8 * q); w[j] = x; }
-      return classify_chunk(w, k * 32, (int64_t)n, at, cls_tbl, KIND);
-    };
-    auto dsat = [&](int64_t k) -> uint32_t { return (k >= 0 && k < n_chunks) ? DS[k] : 0u; };
-    ChunkMasks p = masks(c - 1), o = masks(c), x = masks(c + 1);
-    Window w;
-    w.lead = win(p.lead, o.lead, x.lead); w.L = win(p.L, o.L, x.L); w.N = win(p.N, o.N, x.N); w.S = win(p.S, o.S, x.S);
-    w.SP = win(p.SP, o.SP, x.SP); w.NL = win(p.NL, o.NL, x.NL); w.AP = win(p.AP, o.AP, x.AP);
-    w.DS = win(dsat(c - 1), dsat(c), dsat(c + 1));
-    BoundaryOut r;
-    if (KIND == PT_GPT2) r = boundaries_gpt2(w, c * 32 - 16, at);
-    else r = boundaries_whitespace(w);
-    *drop = r.drop;
-    return r.start;
-  };
   Overflow ov_in; ov_in.bits = 0u;
   uint64_t nfb = 0;
   for (int64_t c = 0; c < n_chunks; ++c) {
@@ -122,10 +101,8 @@ static void emul_fast(const uint8_t* bytes, uint64_t n, const uint64_t* doc_off,
       start = finalize_gpt2(start, m.lead, m.S >> 31, x.lead & 15u, x.S & 15u, DS[c + 1]);
       if (start != before && (m.hi >> 31)) ++nfb;   // counts the straddling multi-byte spaces that were given back
     }
-    (void)exact;
     start_bits[c] = start;
     if (drop_bits) drop_bits[c] = drop;
-    if (planes_out) { uint32_t* d = planes_out + c * 8; d[0] = m.lead; d[1] = m.cont; d[2] = m.L; d[3] = m.N; d[4] = m.S; d[5] = m.SP; d[6] = PT[c].L; d[7] = start; }
     ov_in = o.ov;
   }
   if (fallbacks_out) *fallbacks_out = nfb;
@@ -138,12 +115,6 @@ extern "C" int b2t_emul_pretok_fast(int kind, const uint8_t* bytes, uint64_t n, 
   else if (kind == PT_NOREGEX) emul_fast<PT_NOREGEX>(bytes, n, doc_off, n_docs, cls_tbl, start_bits, drop_bits, fallbacks);
   else if (kind == PT_BERT) emul_fast<PT_BERT>(bytes, n, doc_off, n_docs, cls_tbl, start_bits, drop_bits, fallbacks);
   else return 1;
-  return 0;
-}
-
-extern "C" int b2t_emul_fast_planes(const uint8_t* bytes, uint64_t n, const uint64_t* doc_off, uint32_t n_docs, const uint32_t* cls_tbl,
-                                    uint32_t* start_bits, uint32_t* planes_out) {
-  emul_fast<PT_GPT2>(bytes, n, doc_off, n_docs, cls_tbl, start_bits, nullptr, nullptr, planes_out);
   return 0;
 }
 

@@ -49,11 +49,6 @@ static int fail(int code, const char* fmt, ...) {
 extern "C" const char* b2t_last_error(void) { return g_err; }
 extern "C" const char* b2t_version(void) { return "tokenizers_b200 0.1 (sm_90a)"; }
 
-#ifdef B2T_K1_DEBUG
-extern "C" int b2t_debug_k1(uint32_t* out, size_t words) {
-  return (int)cudaMemcpyFromSymbol(out, b2t::g_k1_dbg, words * 4);
-}
-#endif
 extern "C" int b2t_bert_normalizer_images(int32_t flags, uint8_t* pool, size_t cap, uint32_t* off) {
   if (!pool || !off) return fail(B2T_ERR_INVALID, "b2t_bert_normalizer_images: null argument");
   NormHost nh;
@@ -169,10 +164,7 @@ struct b2t_result {
   void release_host() { h_ids.release(); h_offsets.release(); h_word_ids.release(); h_row_ptr.release(); h_dense_ids.release(); h_dense_mask.release(); h_row_len.release(); }
 };
 
-#ifndef B2T_NSLOT
-#define B2T_NSLOT 3
-#endif
-constexpr int NSLOT = B2T_NSLOT;   // chunk workspaces of one host-path call: NSLOT - 1 chunks are in flight while the next is issued
+constexpr int NSLOT = 3;   // chunk workspaces of one host-path call: NSLOT - 1 chunks are in flight while the next is issued
 constexpr int MAX_KERNEL_RECORDS = 16;
 
 struct b2t_engine {
@@ -180,7 +172,6 @@ struct b2t_engine {
   int model = 0, pretok = 0, add_prefix_space = 0;
   int sm_count = 132;
   int wcache_on = 1;         // B2T_WCACHE=0: no word cache, every pre-token is merged (the reference benches cache_capacity(0) too)
-  int k1_tiled = 0;          // B2T_K1_TILED=1: the round-1 shared-memory-tiled scan (kept for A/B runs)
   DeviceTables dt;
   int monotone = 0;
   DevBuf d_cls, d_byte_to_id, d_merge, d_word, d_pool, d_edge, d_tok2, d_tri;
@@ -264,8 +255,6 @@ extern "C" int b2t_engine_create(const b2t_config* cfg, b2t_engine** out) {
   b2t_engine* e = new b2t_engine();
   e->device = dev; e->model = cfg->model; e->pretok = cfg->pretok; e->add_prefix_space = cfg->add_prefix_space;
   cudaDeviceGetAttribute(&e->sm_count, cudaDevAttrMultiProcessorCount, dev);
-  if (const char* kt = getenv("B2T_K1_TILED")) e->k1_tiled = atoi(kt) != 0;
-  if (cfg->pretok == B2T_PRETOK_BERT) e->k1_tiled = 0;   // (the round-1 tiled scan knows no Bert pre-tokenizer)
   if (const char* wc = getenv("B2T_WCACHE")) e->wcache_on = atoi(wc) != 0;
   if (const char* cb = getenv("B2T_CHUNK_BYTES")) {  // host-path chunk size (tests use tiny chunks to exercise the pipeline)
     long long v = atoll(cb);
@@ -351,51 +340,37 @@ static int ensure_long_pool(Workspace& ws, unsigned long long bytes) {
   return B2T_OK;
 }
 
-#ifndef B2T_K1_TC
-#define B2T_K1_TC 256
-#endif
 template <int KIND>
 static void launch_pretok(b2t_engine* e, const uint8_t* d_bytes, int64_t n, Workspace& ws, cudaStream_t st, bool added) {
-  constexpr int TC = B2T_K1_TC;
+  // every warp owns a contiguous range of whole pages; ~4 waves of resident warps
   const int64_t n_chunks = n / CHUNK + 1;
-  if (!e->k1_tiled) {
-    // streaming form: every warp owns a contiguous range of whole pages; ~4 waves of resident warps
-    const int64_t n_kb = (n_chunks + 31) / 32;
-    const int64_t resident = (int64_t)e->sm_count * (KIND == PT_LLAMA3 ? B2T_K1W_MINBLOCKS : B2T_K1S_MINBLOCKS) * (B2T_K1S_THREADS / 32);
-    int64_t kb = (n_kb + resident * 4 - 1) / (resident * 4);
-    kb = std::min<int64_t>(128, std::max<int64_t>(2, (kb + 1) & ~1ll));
-    const int64_t n_warps = (n_kb + kb - 1) / kb;
-    const int64_t grid = (n_warps + (B2T_K1S_THREADS / 32) - 1) / (B2T_K1S_THREADS / 32);
-    const AddedBits ab{ws.hard_bits.as<uint32_t>(), ws.inner_bits.as<uint32_t>(), ws.added_bits.as<uint32_t>()};
-    if constexpr (KIND == PT_LLAMA3) {
-      if (added)
-        pretok_stream_kernel<KIND, true><<<(unsigned)grid, B2T_K1S_THREADS, 0, st>>>(d_bytes, n, ws.doc_bits.as<uint32_t>(), e->d_cls.as<uint32_t>(),
-                                                                                   ws.start_bits.as<uint32_t>(), ws.drop_bits.as<uint32_t>(),
-                                                                                   ws.page_sum.as<uint64_t>(), (int)n_kb, (int)kb, ab);
-      else
-        pretok_stream_kernel<KIND><<<(unsigned)grid, B2T_K1S_THREADS, 0, st>>>(d_bytes, n, ws.doc_bits.as<uint32_t>(), e->d_cls.as<uint32_t>(),
-                                                                             ws.start_bits.as<uint32_t>(), ws.drop_bits.as<uint32_t>(),
-                                                                             ws.page_sum.as<uint64_t>(), (int)n_kb, (int)kb);
-    } else {
-      const SwapMasks masks{0x55555555u, 0x33333333u, 0x0F0F0F0Fu};
-      if (added)
-        pretok_lean_kernel<KIND, true><<<(unsigned)grid, B2T_K1S_THREADS, 0, st>>>(d_bytes, n, ws.doc_bits.as<uint32_t>(), e->d_cls.as<uint32_t>(),
-                                                                                 ws.start_bits.as<uint32_t>(), ws.drop_bits.as<uint32_t>(),
-                                                                                 ws.page_sum.as<uint64_t>(), (int)n_kb, (int)kb, masks, ab);
-      else
-        pretok_lean_kernel<KIND><<<(unsigned)grid, B2T_K1S_THREADS, 0, st>>>(d_bytes, n, ws.doc_bits.as<uint32_t>(), e->d_cls.as<uint32_t>(),
-                                                                           ws.start_bits.as<uint32_t>(), ws.drop_bits.as<uint32_t>(),
-                                                                           ws.page_sum.as<uint64_t>(), (int)n_kb, (int)kb, masks);
-    }
-    return;
+  const int64_t n_kb = (n_chunks + 31) / 32;
+  const int64_t resident = (int64_t)e->sm_count * (KIND == PT_LLAMA3 ? K1_WINDOW_MINBLOCKS : K1_LEAN_MINBLOCKS) * (K1_THREADS / 32);
+  int64_t kb = (n_kb + resident * 4 - 1) / (resident * 4);
+  kb = std::min<int64_t>(128, std::max<int64_t>(2, (kb + 1) & ~1ll));
+  const int64_t n_warps = (n_kb + kb - 1) / kb;
+  const int64_t grid = (n_warps + (K1_THREADS / 32) - 1) / (K1_THREADS / 32);
+  const AddedBits ab{ws.hard_bits.as<uint32_t>(), ws.inner_bits.as<uint32_t>(), ws.added_bits.as<uint32_t>()};
+  if constexpr (KIND == PT_LLAMA3) {
+    if (added)
+      pretok_stream_kernel<KIND, true><<<(unsigned)grid, K1_THREADS, 0, st>>>(d_bytes, n, ws.doc_bits.as<uint32_t>(), e->d_cls.as<uint32_t>(),
+                                                                            ws.start_bits.as<uint32_t>(), ws.drop_bits.as<uint32_t>(),
+                                                                            ws.page_sum.as<uint64_t>(), (int)n_kb, (int)kb, ab);
+    else
+      pretok_stream_kernel<KIND><<<(unsigned)grid, K1_THREADS, 0, st>>>(d_bytes, n, ws.doc_bits.as<uint32_t>(), e->d_cls.as<uint32_t>(),
+                                                                      ws.start_bits.as<uint32_t>(), ws.drop_bits.as<uint32_t>(),
+                                                                      ws.page_sum.as<uint64_t>(), (int)n_kb, (int)kb);
+  } else {
+    const SwapMasks masks{0x55555555u, 0x33333333u, 0x0F0F0F0Fu};
+    if (added)
+      pretok_lean_kernel<KIND, true><<<(unsigned)grid, K1_THREADS, 0, st>>>(d_bytes, n, ws.doc_bits.as<uint32_t>(), e->d_cls.as<uint32_t>(),
+                                                                          ws.start_bits.as<uint32_t>(), ws.drop_bits.as<uint32_t>(),
+                                                                          ws.page_sum.as<uint64_t>(), (int)n_kb, (int)kb, masks, ab);
+    else
+      pretok_lean_kernel<KIND><<<(unsigned)grid, K1_THREADS, 0, st>>>(d_bytes, n, ws.doc_bits.as<uint32_t>(), e->d_cls.as<uint32_t>(),
+                                                                    ws.start_bits.as<uint32_t>(), ws.drop_bits.as<uint32_t>(),
+                                                                    ws.page_sum.as<uint64_t>(), (int)n_kb, (int)kb, masks);
   }
-  const int64_t n_tiles = (n_chunks + TC - 1) / TC;
-  // contiguous tile ranges per block (the kernel pipelines consecutive tiles); ~8 blocks per SM
-  int64_t tiles_per_block = std::max<int64_t>(1, (n_tiles + (int64_t)e->sm_count * 8 - 1) / ((int64_t)e->sm_count * 8));
-  int64_t grid = (n_tiles + tiles_per_block - 1) / tiles_per_block;
-  pretok_scan_kernel<KIND, TC><<<(unsigned)grid, TC, 0, st>>>(d_bytes, n, ws.doc_bits.as<uint32_t>(), e->d_cls.as<uint32_t>(),
-                                                             ws.start_bits.as<uint32_t>(), ws.drop_bits.as<uint32_t>(),
-                                                             ws.page_sum.as<uint64_t>(), n_tiles, tiles_per_block, 1u);
 }
 
 static void rec(b2t_engine* e, cudaStream_t st, const char* name) {
@@ -776,7 +751,6 @@ extern "C" int b2t_engine_set_added_tokens(b2t_engine* e, uint32_t n_tokens, con
   if (n_tokens == 0) return B2T_OK;
   if (!bytes || !off || !ids || !flags) return fail(B2T_ERR_INVALID, "b2t_engine_set_added_tokens: null argument");
   if (e->add_prefix_space) return fail(B2T_ERR_UNSUPPORTED, "added-token extraction on the device does not combine with add_prefix_space");
-  if (e->k1_tiled) return fail(B2T_ERR_UNSUPPORTED, "added-token extraction needs the streaming scan kernels");
   if (e->norm_on) return fail(B2T_ERR_UNSUPPORTED, "added-token extraction on the device runs on the text the engine is given: with a normalizer the host splits first");
   // two sets (normalized == false first), longest token first inside a set (find_matches: leftmost-longest)
   std::vector<uint32_t> order[2];

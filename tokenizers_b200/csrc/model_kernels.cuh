@@ -330,11 +330,9 @@ __device__ __forceinline__ void coop_bpe(const DeviceTables& t, const uint8_t* s
 }
 
 
-#ifndef B2T_MINBLOCKS
-#define B2T_MINBLOCKS 8  // 8 blocks/SM (32 regs, small spills) rather than 5 (48 regs): the kernel is latency-bound
-#endif
+constexpr int MODEL_MINBLOCKS = 8;  // 8 blocks/SM (32 regs, small spills) rather than 5 (48 regs): the kernel is latency-bound
 template <int MODEL>
-__global__ void __launch_bounds__(MODEL_THREADS, B2T_MINBLOCKS) model_tile_kernel(const ModelParams P) {
+__global__ void __launch_bounds__(MODEL_THREADS, MODEL_MINBLOCKS) model_tile_kernel(const ModelParams P) {
   constexpr int HALO = MODEL == MODEL_BPE ? 256 : 416;
   constexpr int SPAN = TILE + HALO;
   constexpr int NW = SPAN / 32;

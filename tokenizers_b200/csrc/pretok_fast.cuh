@@ -1,6 +1,6 @@
 // pretok_fast.cuh -- bit-sliced classification and 32-bit boundary algebra of the pre-tokenization scan (host + device).
 //
-// This is the fast path of K1 (pretok_stream_kernel in pretok_kernels.cuh).  It computes exactly what the window code of
+// This is the fast path of K1 (the streaming kernels of pretok_kernels.cuh).  It computes exactly what the window code of
 // pretok_logic.cuh computes -- the split points of
 //   pre_tokenizers/byte_level.rs:43-46,119-131 (GPT-2 pattern), pre_tokenizers/whitespace.rs:20-29 (\w+|[^\w\s]+)
 // -- with about a third of the instructions, because the kernel is bound by the integer pipe, not by HBM:
@@ -12,8 +12,8 @@
 //      the rest take a table look-up per character (resolve_uncertain);
 //   3. the boundary predicates work on the chunk's own 32-bit masks, the neighbours contribute single bits
 //      (funnel shifts) instead of 64-bit windows.
-// The window code stays as the exact fallback for the one case the fast algebra does not cover (a multi-byte
-// whitespace character that straddles the chunk end) and as the Llama-3 algebra.
+// The window code stays as the Llama-3 algebra.  The one case the fast GPT-2 algebra leaves open (a whitespace character
+// that ends the chunk or straddles its end) is settled by finalize_gpt2 with the next chunk's first bits.
 // Everything here is pure so that tests/native/pretok_emul.cpp runs exactly this code on the CPU.
 #pragma once
 #include "pretok_logic.cuh"
@@ -35,19 +35,9 @@ B2T_HD uint32_t bperm(uint32_t x, uint32_t y, uint32_t s) {
 B2T_HD uint32_t fsl(uint32_t lo, uint32_t hi, int k) { return (uint32_t)(((((uint64_t)hi << 32) | lo) << k) >> 32); }
 B2T_HD uint32_t fsr(uint32_t lo, uint32_t hi, int k) { return (uint32_t)((((uint64_t)hi << 32) | lo) >> k); }
 #endif
-// x >> K for a constant K.  On the device as a multiply-high: the shift units share the integer pipe with the logic
-// ops that bound this kernel, the multiplier sits on the other pipe (kept switchable, off by default).
-#ifndef B2T_SHR_MULHI
-#define B2T_SHR_MULHI 0
-#endif
+// x >> K for a constant K
 template <int K>
-B2T_HD uint32_t shr(uint32_t x) {
-#if defined(__CUDA_ARCH__) && B2T_SHR_MULHI
-  return __umulhi(x, 1u << (32 - K));
-#else
-  return x >> K;
-#endif
-}
+B2T_HD uint32_t shr(uint32_t x) { return x >> K; }
 // 3-input look-up: bit (a b c) of TB.  Written as a sum of minterms over three variables, which nvcc folds into ONE LOP3.
 // (An inline-asm lop3 here once produced wrong class masks when the call sat next to a warp vote -- seen on the GPU
 // against the CPU run of this very file -- so the compiler does the folding.)

@@ -1,4 +1,5 @@
-// pretok_kernels.cuh -- K0 doc_mark, K1 pretok_scan (the HBM-roofline-graded kernel), K1b page_scan.
+// pretok_kernels.cuh -- K0 doc_mark, K1 pre-tokenization scan (pretok_lean_kernel / pretok_stream_kernel, the
+// HBM-roofline-graded kernel), K1b page_scan.
 //
 // Data layout in HBM (one batch = `n` packed UTF-8 bytes, documents back to back):
 //   bytes      u8 [n]                input, read once by K1 with 16-byte loads
@@ -82,204 +83,6 @@ __device__ __forceinline__ uint64_t pack_sum(uint32_t tot, uint32_t aft, uint32_
   // tot / aft carry two 16-bit fields each (chars | splits << 16)
   return (uint64_t)(tot & 0xFFFu) | ((uint64_t)((tot >> 16) & 0xFFFu) << 12) | ((uint64_t)(aft & 0xFFFu) << 24) |
          ((uint64_t)((aft >> 16) & 0xFFFu) << 36) | ((uint64_t)(flag & 1u) << 48);
-}
-
-// K1.  Each block owns a contiguous range of tiles (TC chunks = TC * 32 bytes each) and software-pipelines them:
-// phase A of tile t+1 (class masks -> shared memory) runs before phase B of tile t (boundaries from the 64-byte
-// windows), so the halo chunk on the right comes for free and the one on the left is kept from the previous tile.
-//   A1  per lane: 2 x 16-byte loads, ASCII masks by SWAR (ascii_masks), store to shared memory
-//   A2  per warp: the non-ASCII characters of the warp's 1 KB are compacted into a list and classified by all 32
-//       lanes together (decode + 2-bit class table), results OR-ed into the owners' masks with shared atomics --
-//       no lane diverges on "my chunk has 10 Cyrillic letters and yours has none"
-//   B   per lane: windows from the neighbours' masks, boundary algebra (pretok_logic.cuh), 4-byte store of the bitmap
-//       word, page summaries by warp reductions
-#ifndef B2T_K1_MINBLOCKS
-#define B2T_K1_MINBLOCKS 4
-#endif
-template <int KIND, int TC>
-__global__ void __launch_bounds__(TC, B2T_K1_MINBLOCKS) pretok_scan_kernel(const uint8_t* __restrict__ bytes, int64_t n,
-                                                         const uint32_t* __restrict__ doc_bits,
-                                                         const uint32_t* __restrict__ cls_tbl,
-                                                         uint32_t* __restrict__ start_bits, uint32_t* __restrict__ drop_bits,
-                                                         uint64_t* __restrict__ page_sum, int64_t n_tiles, int64_t tiles_per_block, uint32_t one) {
-  constexpr int NWARPS = TC / 32;
-  __shared__ ChunkMasks sm[2][TC];
-  __shared__ ChunkMasks sm_prev;                 // last chunk of the tile before the one in phase B
-  __shared__ uint32_t s_spill[2][NWARPS][4];     // class bits spilling from a warp's last chunk into the next warp's first
-  __shared__ uint16_t s_list[NWARPS][512];       // positions (within the warp's 1 KB) of its non-ASCII lead bytes
-  __shared__ uint32_t s_wsum[NWARPS * 3];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int64_t n_chunks = n / CHUNK + 1;
-  ByteAtGlobal at{bytes, n};
-  DsAtGlobal dsat{doc_bits, n_chunks};
-  const int64_t t_lo = (int64_t)blockIdx.x * tiles_per_block;
-  const int64_t t_hi = (t_lo + tiles_per_block < n_tiles) ? t_lo + tiles_per_block : n_tiles;
-  if (t_lo >= t_hi) return;
-
-  // ---- phase A of one tile into buffer `buf`
-  auto phase_a = [&](int64_t tile, int buf) {
-    const int64_t c = tile * TC + tid, base = c * CHUNK;
-    ChunkMasks m;
-    uint32_t hi = 0, cont = 0;
-    if (base < n) {
-      uint32_t w[8];
-      load_chunk_words(bytes, base, n, w);
-      ascii_masks(KIND, w, m, &hi, &cont, one);
-      if (base + CHUNK > n) {
-        const uint32_t valid = 0xFFFFFFFFu >> (32 - (int)(n - base));
-        m.lead &= valid; hi &= valid; cont &= valid;
-      }
-    } else { m.lead = m.L = m.N = m.S = m.SP = m.NL = m.AP = 0u; }
-    sm[buf][tid] = m;
-    // my OUTGOING spill slot (the incoming one may be written by the warp below at any time; slot 0 stays zero)
-    if (lane < 4 && warp + 1 < NWARPS) s_spill[buf][warp + 1][lane] = 0u;
-    __syncwarp();
-    if (__any_sync(0xFFFFFFFFu, hi != 0u)) {
-      // A2: compact the warp's non-ASCII lead bytes, then classify them with all lanes
-      uint32_t nl = hi & ~cont;
-      const int cnt = __popc(nl);
-      int inc = cnt;
-#pragma unroll
-      for (int st = 1; st < 32; st <<= 1) { int o = __shfl_up_sync(0xFFFFFFFFu, inc, st); if (lane >= st) inc += o; }
-      const int total = __shfl_sync(0xFFFFFFFFu, inc, 31);
-      int off = inc - cnt;
-      while (nl) { s_list[warp][off++] = (uint16_t)(lane * 32 + __ffs((int)nl) - 1); nl &= nl - 1u; }
-      // a character that started in the previous TILE owns my first bytes (tid 0 only; inside the tile the owner
-      // of the lead byte spills its bits into the neighbour below)
-      if (tid == 0 && (cont & 1u)) {
-        int back = 1;
-        while (back < 3 && (at(base - back) & 0xC0u) == 0x80u) ++back;
-        int len;
-        const int64_t q = base - back;
-        const uint32_t cl = decode_class(at(q), at(q + 1), at(q + 2), at(q + 3), cls_tbl, &len);
-        const int cover = len - back;
-        if (cover > 0 && cl != CLS_O) atomicOr(reinterpret_cast<uint32_t*>(&sm[buf][0]) + cl, (1u << cover) - 1u);
-      }
-      __syncwarp();
-      const uint32_t wbase = (uint32_t)((tile * TC + warp * 32) * CHUNK);   // batches are < 2^31 bytes
-      const uint32_t* __restrict__ words = reinterpret_cast<const uint32_t*>(bytes);
-      uint32_t* smw = reinterpret_cast<uint32_t*>(&sm[buf][warp * 32]);
-      constexpr int STRIDE = sizeof(ChunkMasks) / 4;
-      for (int i = lane; i < total; i += 32) {
-        const uint32_t idx = s_list[warp][i];
-        const uint32_t gp = wbase + idx;
-        const uint32_t a0 = __ldg(words + (gp >> 2)), a1 = ((gp | 3u) + 1u < (uint32_t)n) ? __ldg(words + (gp >> 2) + 1) : 0u;
-        const uint32_t v = __funnelshift_r(a0, a1, (gp & 3u) * 8u);
-        const uint32_t b0 = v & 0xFFu;
-        const int len = 2 + (b0 >= 0xE0u) + (b0 >= 0xF0u);
-        // branch-free decode (the three lengths are mixed inside a warp): the low 6 bits of all four bytes as if the
-        // character had 4 bytes, shifted down by the bytes it does not have, lead-byte marker bits masked off
-        const uint32_t t24 = ((v & 0x3Fu) << 18) | ((v << 4) & 0x3F000u) | ((v >> 10) & 0xFC0u) | ((v >> 24) & 0x3Fu);
-        uint32_t cp = (t24 >> (6 * (4 - len))) & ((2u << (5 * len)) - 1u);
-        cp = cp < 0x110000u ? cp : 0x10FFFFu;
-        const uint32_t cl = (__ldg(cls_tbl + (cp >> 4)) >> ((cp & 15u) * 2u)) & 3u;
-        if (cl != CLS_O) {
-          const uint32_t owner = idx >> 5, p = idx & 31u, m = (1u << len) - 1u;
-          atomicOr(smw + owner * STRIDE + cl, m << p);
-          if (p + (uint32_t)len > 32u) {
-            const uint32_t hi32 = m >> (32u - p);
-            if (owner < 31u) atomicOr(smw + (owner + 1u) * STRIDE + cl, hi32);
-            else if (warp + 1 < NWARPS) atomicOr(&s_spill[buf][warp + 1][cl], hi32);
-          }
-        }
-      }
-    }
-  };
-  auto load_masks = [&](int buf, int idx) -> ChunkMasks {
-    ChunkMasks m = sm[buf][idx];
-    if ((idx & 31) == 0) { const uint32_t* sp = s_spill[buf][idx >> 5]; m.L |= sp[CLS_L]; m.N |= sp[CLS_N]; m.S |= sp[CLS_S]; }
-    return m;
-  };
-
-  // ---- prologue
-  if (tid < 8) s_spill[tid >> 2][0][tid & 3] = 0u;
-  if (tid == 0) {
-    sm_prev = classify_global<KIND>(bytes, n, t_lo * TC - 1, cls_tbl);
-  }
-  phase_a(t_lo, (int)(t_lo & 1));
-
-  for (int64_t tile = t_lo; tile < t_hi; ++tile) {
-    const int buf = (int)(tile & 1), nbuf = buf ^ 1;
-    if (tile + 1 < t_hi) phase_a(tile + 1, nbuf);
-    else if (tid == 0) {  // first chunk after my range (phase B of my last tile looks 16 bytes into it)
-      sm[nbuf][0] = classify_global<KIND>(bytes, n, (tile + 1) * TC, cls_tbl);
-    }
-    __syncthreads();
-    // ---- phase B
-    const int64_t c = tile * TC + tid;
-    BoundaryOut r;
-    ChunkMasks o = load_masks(buf, tid);
-    // doc-start words of chunks c-1, c, c+1 (chunk indices fit 32 bits: batches are < 2^31 bytes; c - 1 wraps to "outside")
-    auto ds32 = [&](uint32_t k) -> uint32_t { return k < (uint32_t)n_chunks ? __ldg(doc_bits + k) : 0u; };
-    const uint32_t own_ds = ds32((uint32_t)c);
-    {
-      const ChunkMasks p = tid == 0 ? sm_prev : load_masks(buf, tid - 1);
-      const ChunkMasks x = tid == TC - 1 ? load_masks(nbuf, 0) : load_masks(buf, tid + 1);
-      Window w;
-      w.lead = win(p.lead, o.lead, x.lead); w.L = win(p.L, o.L, x.L); w.N = win(p.N, o.N, x.N); w.S = win(p.S, o.S, x.S);
-      w.SP = win(p.SP, o.SP, x.SP); w.NL = KIND == PT_LLAMA3 ? win(p.NL, o.NL, x.NL) : 0ull; w.AP = win(p.AP, o.AP, x.AP);
-      w.DS = win(ds32((uint32_t)c - 1u), own_ds, ds32((uint32_t)c + 1u));
-      const int64_t wb = c * CHUNK - 16;
-      if (KIND == PT_GPT2) {
-        r = boundaries_gpt2(w, wb, at);
-      } else if (KIND == PT_LLAMA3) {
-        LlamaCarry cy; cy.n_count_before_window = 0; cy.zone_before_window = false; cy.tail_after_window = false;
-        r = boundaries_llama3(w, wb, at, cy);
-        if (r.slow) {
-          // rare: a run reaches beyond the window; the carry walks chunk masks re-classified from global memory
-          struct GlobalMaskAt {
-            const uint8_t* bytes; int64_t n; const uint32_t* cls;
-            __device__ __forceinline__ ChunkMasks operator()(int64_t k) const { return classify_global<KIND>(bytes, n, k, cls); }
-          } masks{bytes, n, cls_tbl};
-          cy = llama_carry(c, n_chunks, masks, dsat);
-          r = boundaries_llama3(w, wb, at, cy);
-        }
-      } else if (KIND == PT_WHITESPACE) {
-        r = boundaries_whitespace(w);
-      } else {
-        r.start = (uint32_t)((w.DS & w.lead) >> 16); r.drop = 0; r.slow = 0;
-      }
-    }
-    if (c < n_chunks) {
-      start_bits[c] = r.start;
-      if (KIND == PT_WHITESPACE) drop_bits[c] = r.drop;
-    }
-    // ---- page summaries (segmented: counts restart at the last doc start of the page), warp reductions
-    {
-      const uint32_t kept = r.start & ~r.drop;
-      const uint32_t tot = (uint32_t)__popc(o.lead) | ((uint32_t)__popc(kept) << 16);
-      const unsigned dsm = __ballot_sync(0xFFFFFFFFu, own_ds != 0u);
-      const uint32_t wtot = __reduce_add_sync(0xFFFFFFFFu, tot);
-      uint32_t waft = 0;
-      if (dsm) {
-        const int last = 31 - __clz((int)dsm);
-        uint32_t mine = 0;
-        if (lane > last) mine = tot;
-        else if (lane == last) {
-          const uint32_t from = ~bits_below(31 - __clz((int)own_ds));
-          mine = (uint32_t)__popc(o.lead & from) | ((uint32_t)__popc(kept & from) << 16);
-        }
-        waft = __reduce_add_sync(0xFFFFFFFFu, mine);
-      }
-      if (lane == 0) { s_wsum[warp * 3] = wtot; s_wsum[warp * 3 + 1] = waft; s_wsum[warp * 3 + 2] = dsm != 0u; }
-    }
-    __syncthreads();  // all reads of sm[buf] / sm_prev are done; s_wsum is complete
-    {
-      constexpr int WPP = PAGE_CHUNKS / 32;  // warps per page (2)
-      if (tid < NWARPS / WPP) {
-        uint32_t t0 = s_wsum[(tid * WPP) * 3], a0 = s_wsum[(tid * WPP) * 3 + 1], f0 = s_wsum[(tid * WPP) * 3 + 2];
-#pragma unroll
-        for (int k = 1; k < WPP; ++k) {
-          uint32_t t1 = s_wsum[(tid * WPP + k) * 3], a1 = s_wsum[(tid * WPP + k) * 3 + 1], f1 = s_wsum[(tid * WPP + k) * 3 + 2];
-          a0 = f1 ? a1 : a0 + t1; t0 += t1; f0 |= f1;
-        }
-        const int64_t page = tile * (TC / PAGE_CHUNKS) + tid;
-        if (page * PAGE <= n) page_sum[page] = pack_sum(t0, a0, f0);
-      }
-      if (tid == TC - 1) sm_prev = o;
-    }
-    // the next iteration's phase A writes sm[buf] and s_wsum is rewritten only after the next barrier
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ K1b
@@ -373,8 +176,9 @@ __global__ void __launch_bounds__(SCAN_BLOCK) page_scan_top_kernel(const uint64_
 
 }  // namespace b2t
 
-// ================================================================================================ K1, streaming form
-// pretok_stream_kernel: the production K1.  Every WARP streams through its own contiguous range of the batch, 1 KB
+// ================================================================================================ K1
+// pretok_lean_kernel (GPT-2, Whitespace, Bert, no regex) and pretok_stream_kernel (Llama-3), one kernel per
+// pre-tokenizer with the same streaming structure.  Every WARP streams through its own contiguous range of the batch, 1 KB
 // (32 chunks of 32 bytes, one per lane) per iteration, and is independent of all other warps: no shared memory, no
 // block barrier.  Iteration i+1 is classified (pretok_fast.cuh: bit planes -> classes) before the boundaries of
 // iteration i are evaluated, so a lane gets everything it needs from its neighbours with warp shuffles:
@@ -386,11 +190,12 @@ __global__ void __launch_bounds__(SCAN_BLOCK) page_scan_top_kernel(const uint64_
 
 namespace b2t {
 
-// Exact window code (pretok_logic.cuh) for one chunk, everything re-read from global memory.  Used by the rare
-// fallback of the fast GPT-2 algebra and as the Llama-3 slow path.
+// The Llama-3 slow path: the exact window code (pretok_logic.cuh) for one chunk whose runs reach beyond its window,
+// everything re-read from global memory and the carry walked over chunk masks re-classified from there.
 template <int KIND>
 __device__ __noinline__ uint32_t exact_chunk_start(const uint8_t* __restrict__ bytes, int64_t n, int64_t c,
                                                   const uint32_t* __restrict__ cls_tbl, const uint32_t* __restrict__ doc_bits) {
+  static_assert(KIND == PT_LLAMA3, "the slow path of the Llama-3 kernel");
   const int64_t n_chunks = n / CHUNK + 1;
   ByteAtGlobal at{bytes, n};
   DsAtGlobal dsat{doc_bits, n_chunks};
@@ -398,34 +203,21 @@ __device__ __noinline__ uint32_t exact_chunk_start(const uint8_t* __restrict__ b
                    x = classify_global<KIND>(bytes, n, c + 1, cls_tbl);
   Window w;
   w.lead = win(p.lead, o.lead, x.lead); w.L = win(p.L, o.L, x.L); w.N = win(p.N, o.N, x.N); w.S = win(p.S, o.S, x.S);
-  w.SP = win(p.SP, o.SP, x.SP); w.NL = KIND == PT_LLAMA3 ? win(p.NL, o.NL, x.NL) : 0ull; w.AP = win(p.AP, o.AP, x.AP);
+  w.SP = win(p.SP, o.SP, x.SP); w.NL = win(p.NL, o.NL, x.NL); w.AP = win(p.AP, o.AP, x.AP);
   w.DS = win(dsat(c - 1), dsat(c), dsat(c + 1));
   const int64_t wb = c * CHUNK - 16;
-  if (KIND == PT_GPT2) return boundaries_gpt2(w, wb, at).start;
-  if (KIND == PT_LLAMA3) {
-    struct GlobalMaskAt {
-      const uint8_t* bytes; int64_t n; const uint32_t* cls;
-      __device__ __forceinline__ ChunkMasks operator()(int64_t k) const { return classify_global<KIND>(bytes, n, k, cls); }
-    } masks{bytes, n, cls_tbl};
-    const LlamaCarry cy = llama_carry(c, n_chunks, masks, dsat);
-    return boundaries_llama3(w, wb, at, cy).start;
-  }
-  return boundaries_whitespace(w).start;
+  struct GlobalMaskAt {
+    const uint8_t* bytes; int64_t n; const uint32_t* cls;
+    __device__ __forceinline__ ChunkMasks operator()(int64_t k) const { return classify_global<KIND>(bytes, n, k, cls); }
+  } masks{bytes, n, cls_tbl};
+  const LlamaCarry cy = llama_carry(c, n_chunks, masks, dsat);
+  return boundaries_llama3(w, wb, at, cy).start;
 }
 
-#ifndef B2T_K1S_THREADS
-#define B2T_K1S_THREADS 128
-#endif
-#ifndef B2T_K1S_MINBLOCKS
-#define B2T_K1S_MINBLOCKS 8
-#endif
-#ifndef B2T_K1W_MINBLOCKS
-#define B2T_K1W_MINBLOCKS 4   // window (Llama-3) form: more live state
-#endif
+constexpr int K1_THREADS = 128;
+constexpr int K1_LEAN_MINBLOCKS = 8;
+constexpr int K1_WINDOW_MINBLOCKS = 4;   // window (Llama-3) form: more live state
 
-#ifdef B2T_K1_DEBUG
-__device__ uint32_t g_k1_dbg[8192 * 8];
-#endif
 // byte access with 32-bit positions (batches are < 2^31 bytes; "negative" positions wrap to out-of-range)
 struct ByteAt32 {
   const uint8_t* __restrict__ p;
@@ -467,7 +259,7 @@ __device__ __forceinline__ void load_tail_words(const uint8_t* __restrict__ byte
 // span's bytes (added_bits | inner_bits).  The page summaries keep counting from the DOCUMENT starts.
 struct AddedBits { const uint32_t* hard; const uint32_t* inner; const uint32_t* added; };
 template <int KIND, bool ADDED = false>
-__global__ void __launch_bounds__(B2T_K1S_THREADS, B2T_K1S_MINBLOCKS)
+__global__ void __launch_bounds__(K1_THREADS, K1_LEAN_MINBLOCKS)
 pretok_lean_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint32_t* __restrict__ doc_bits,
                    const uint32_t* __restrict__ cls_tbl, uint32_t* __restrict__ start_bits, uint32_t* __restrict__ drop_bits,
                    uint64_t* __restrict__ page_sum, int n_kb, int kb_per_warp, SwapMasks masks, AddedBits ab = AddedBits{nullptr, nullptr, nullptr}) {
@@ -605,9 +397,10 @@ pretok_lean_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint32_
 }
 
 // ---------------------------------------------------------------------------------------------- window form (Llama-3)
-// Same streaming structure with the 64-bit window algebra of pretok_logic.cuh (two iterations per trip).
+// Same streaming structure with the 64-bit window algebra of pretok_logic.cuh (two iterations per trip).  drop_bits is
+// not written: the tiktoken pattern removes nothing, every split is kept.
 template <int KIND, bool ADDED = false>
-__global__ void __launch_bounds__(B2T_K1S_THREADS, B2T_K1W_MINBLOCKS)
+__global__ void __launch_bounds__(K1_THREADS, K1_WINDOW_MINBLOCKS)
 pretok_stream_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint32_t* __restrict__ doc_bits,
                      const uint32_t* __restrict__ cls_tbl, uint32_t* __restrict__ start_bits, uint32_t* __restrict__ drop_bits,
                      uint64_t* __restrict__ page_sum, int n_kb, int kb_per_warp, AddedBits ab = AddedBits{nullptr, nullptr, nullptr}) {
@@ -642,24 +435,18 @@ pretok_stream_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint3
     uint32_t b[8];
     bitslice32(w, b);
     m = classify_planes<KIND>(b, valid);
-#ifdef B2T_K1_NOANY
-    {
-#else
     if (__any_sync(FULL, m.hi != 0u)) {
-#endif
       if (m.unc) resolve_uncertain(m, at4, base, cls_tbl);
       fill_own(m);
     }
-    // the chunk before mine (only bit 31 of the class words matters to the fast algebra; Llama-3 uses the top halves)
+    // the chunk before mine (the window algebra uses the top halves of its class words)
     pm.L = __shfl_sync(FULL, lane == 31 ? prev.L : m.L, up);
-    pm.N = KIND == PT_WHITESPACE ? 0u : __shfl_sync(FULL, lane == 31 ? prev.N : m.N, up);
+    pm.N = __shfl_sync(FULL, lane == 31 ? prev.N : m.N, up);
     pm.S = __shfl_sync(FULL, lane == 31 ? prev.S : m.S, up);
-    pm.SP = KIND == PT_WHITESPACE ? 0u : __shfl_sync(FULL, lane == 31 ? prev.SP : m.SP, up);
-    if (KIND == PT_LLAMA3) {
-      pm.lead = __shfl_sync(FULL, lane == 31 ? prev.lead : m.lead, up);
-      pm.NL = __shfl_sync(FULL, lane == 31 ? prev.NL : m.NL, up);
-      pm.AP = __shfl_sync(FULL, lane == 31 ? prev.AP : m.AP, up);
-    }
+    pm.SP = __shfl_sync(FULL, lane == 31 ? prev.SP : m.SP, up);
+    pm.lead = __shfl_sync(FULL, lane == 31 ? prev.lead : m.lead, up);
+    pm.NL = __shfl_sync(FULL, lane == 31 ? prev.NL : m.NL, up);
+    pm.AP = __shfl_sync(FULL, lane == 31 ? prev.AP : m.AP, up);
     if (m.cont & 1u) spill_in(m, pm.L, pm.N, pm.S);
   };
 
@@ -676,7 +463,7 @@ pretok_stream_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint3
     const uint32_t ds = c < n_chunks ? __ldg(rbits + c) : 0u;
     const uint32_t ds_next = c + 1 < n_chunks ? __ldg(rbits + c + 1) : 0u;
     const uint32_t docw = ADDED ? (c < n_chunks ? __ldg(doc_bits + c) : 0u) : ds;
-    uint32_t start, drop = 0u;
+    uint32_t start;
     {
       // window algebra of pretok_logic.cuh on [16 B of the previous chunk | mine | 16 B of the next chunk]
       Window wd;
@@ -694,16 +481,9 @@ pretok_stream_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint3
       if (r.slow) start = exact_chunk_start<KIND>(bytes, n64, c, cls_tbl, rbits);
     }
     if (ADDED && c < n_chunks) start &= ~__ldg(ab.inner + c);   // an added token's span is one pre-token
-    if (c < n_chunks) {
-      start_bits[c] = start;
-      if (KIND == PT_WHITESPACE) drop_bits[c] = drop;
-    }
-#ifdef B2T_K1_DEBUG
-    if (c < 8192u) { uint32_t* d = g_k1_dbg + c * 8; d[0] = cur.lead; d[1] = cur.cont; d[2] = cur.L; d[3] = cur.N; d[4] = cur.S; d[5] = cur.SP; d[6] = pcur.L; d[7] = start; }
-#endif
+    if (c < n_chunks) start_bits[c] = start;
     // ---- page summary (segmented: counts restart at the last doc start of the page); this iteration is half a page
-    const uint32_t kept = start & ~drop;
-    const uint32_t tot = (uint32_t)__popc(cur.lead) | ((uint32_t)__popc(kept) << 16);
+    const uint32_t tot = (uint32_t)__popc(cur.lead) | ((uint32_t)__popc(start) << 16);
     const unsigned dsm = __ballot_sync(FULL, docw != 0u);
     const uint32_t wtot = __reduce_add_sync(FULL, tot);
     uint32_t waft = 0u;
@@ -713,7 +493,7 @@ pretok_stream_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint3
       if (lane > last) mine = tot;
       else if (lane == last) {
         const uint32_t from = ~bits_below(31 - __clz((int)docw));
-        mine = (uint32_t)__popc(cur.lead & from) | ((uint32_t)__popc(kept & from) << 16);
+        mine = (uint32_t)__popc(cur.lead & from) | ((uint32_t)__popc(start & from) << 16);
       }
       waft = __reduce_add_sync(FULL, mine);
     }

@@ -93,9 +93,7 @@ B2T_HD uint32_t decode_at(const ByteAt& at, int64_t p, int64_t end, int* len) {
 // characters are rare, so their masks are built in a second pass only when a cheap detector saw one.
 // Outputs: m.L / m.N / m.S / m.SP / m.NL / m.AP for ASCII bytes only, *hi = non-ASCII bytes, *cont = continuation bytes.
 // kind: PT_WHITESPACE uses the Rust-regex classes (\w on ASCII = [0-9A-Za-z_], N slot unused).
-// `one` must be 1 at run time and opaque to the compiler: x * one + c makes the SWAR adds IMADs (FMA pipe) instead of
-// IADD3s, so they no longer compete with the LOP3 / SHF work for the ALU pipe.
-B2T_HD void ascii_masks(int kind, const uint32_t w[8], ChunkMasks& m, uint32_t* hi_out, uint32_t* cont_out, uint32_t one = 1u) {
+B2T_HD void ascii_masks(int kind, const uint32_t w[8], ChunkMasks& m, uint32_t* hi_out, uint32_t* cont_out) {
   const bool rust = kind == PT_WHITESPACE;
   uint32_t L = 0, N = 0, SP = 0, CT = 0, HI = 0, any_ctl = 0, any_ap = 0, any_hi = 0;
 #pragma unroll
@@ -107,13 +105,13 @@ B2T_HD void ascii_masks(int kind, const uint32_t w[8], ChunkMasks& m, uint32_t* 
       const uint32_t asc = ~x & 0x80808080u;            // bit 7 set <=> ASCII byte
       const uint32_t w7 = x & 0x7F7F7F7Fu;
       const uint32_t t = w7 | 0x20202020u;
-      uint32_t l = (t * one + 0x1F1F1F1Fu) & ~(t * one + 0x05050505u) & asc;             // 'a'..'z' after folding case
-      uint32_t d = (w7 * one + 0x50505050u) & ~(w7 * one + 0x46464646u) & asc;           // '0'..'9'
-      if (rust) { l |= d | ((w7 * one + 0x21212121u) & ~(w7 * one + 0x20202020u) & asc); d = 0u; }  // + '_' (0x5F)
+      uint32_t l = (t + 0x1F1F1F1Fu) & ~(t + 0x05050505u) & asc;             // 'a'..'z' after folding case
+      uint32_t d = (w7 + 0x50505050u) & ~(w7 + 0x46464646u) & asc;           // '0'..'9'
+      if (rust) { l |= d | ((w7 + 0x21212121u) & ~(w7 + 0x20202020u) & asc); d = 0u; }  // + '_' (0x5F)
       fL[h] = l; fN[h] = d;
-      fSP[h] = (w7 * one + 0x60606060u) & ~(w7 * one + 0x5F5F5F5Fu) & asc;               // == 0x20
-      any_ctl |= ~(w7 * one + 0x60606060u) & asc;                                   // < 0x20
-      any_ap |= (w7 * one + 0x59595959u) & ~(w7 * one + 0x58585858u) & asc;              // == 0x27
+      fSP[h] = (w7 + 0x60606060u) & ~(w7 + 0x5F5F5F5Fu) & asc;               // == 0x20
+      any_ctl |= ~(w7 + 0x60606060u) & asc;                                   // < 0x20
+      any_ap |= (w7 + 0x59595959u) & ~(w7 + 0x58585858u) & asc;              // == 0x27
       any_hi |= x;
     }
     const int sh = 4 * j;  // 8 mask bits per pair of words
@@ -137,10 +135,10 @@ B2T_HD void ascii_masks(int kind, const uint32_t w[8], ChunkMasks& m, uint32_t* 
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const uint32_t x = w[j + h], asc = ~x & 0x80808080u, w7 = x & 0x7F7F7F7Fu;
-        a[h] = (w7 * one + 0x77777777u) & ~(w7 * one + 0x72727272u) & asc;                // 9..13
+        a[h] = (w7 + 0x77777777u) & ~(w7 + 0x72727272u) & asc;                // 9..13
         b[h] = 0u;
         if (kind == PT_LLAMA3)  // only the tiktoken pattern distinguishes newlines
-          b[h] = (((w7 * one + 0x76767676u) & ~(w7 * one + 0x75757575u)) | ((w7 * one + 0x73737373u) & ~(w7 * one + 0x72727272u))) & asc;  // 10, 13
+          b[h] = (((w7 + 0x76767676u) & ~(w7 + 0x75757575u)) | ((w7 + 0x73737373u) & ~(w7 + 0x72727272u))) & asc;  // 10, 13
       }
       S |= movemask2(a[0], a[1]) << (4 * j);
       if (kind == PT_LLAMA3) NL |= movemask2(b[0], b[1]) << (4 * j);
@@ -153,7 +151,7 @@ B2T_HD void ascii_masks(int kind, const uint32_t w[8], ChunkMasks& m, uint32_t* 
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const uint32_t x = w[j + h], asc = ~x & 0x80808080u, w7 = x & 0x7F7F7F7Fu;
-        a[h] = (w7 * one + 0x59595959u) & ~(w7 * one + 0x58585858u) & asc;
+        a[h] = (w7 + 0x59595959u) & ~(w7 + 0x58585858u) & asc;
       }
       AP |= movemask2(a[0], a[1]) << (4 * j);
     }

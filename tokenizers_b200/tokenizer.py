@@ -7,7 +7,7 @@ Mirrors `tokenizers.Tokenizer` (bindings/python/src/tokenizer.rs:510-1461 in the
 hot path raise `UnsupportedConfig` (there is no CPU fallback).  The two host steps the reference runs around the path are
 mirrored here: added-token extraction before it (`added.py`) and the special-token template after it (`post_process`).
 """
-import ctypes, os, json
+import ctypes, json
 import numpy as np
 from . import _lib, added, pairs
 from ._lib import B2TError
@@ -525,7 +525,7 @@ class Tokenizer:
         if rc == _lib.B2T_ERR_UNSUPPORTED:
             return
         _lib.check(rc)
-        self._dev_added = os.environ.get("B2T_HOST_ADDED", "0") != "1"   # B2T_HOST_ADDED=1: keep the host extraction (A/B, tests)
+        self._dev_added = True
         self._added_strip = any(t.lstrip or t.rstrip for t in toks)
 
     def __del__(self):
