@@ -170,6 +170,180 @@ def with_added_tokens(tokenizer_json, template=False):
     return json.dumps(js)
 
 
+def tokenizer_with_env(tokenizer_json, **env):
+    """tokenizers_b200.Tokenizer created with the engine switches in `env` (B2T_WCACHE, B2T_CHUNK_BYTES: read when the
+    engine is created); the caller's environment is restored afterwards"""
+    from tokenizers_b200 import Tokenizer
+    old = {k: os.environ.get(k) for k in env}
+    os.environ.update({k: str(v) for k, v in env.items()})
+    try:
+        return Tokenizer.from_str(tokenizer_json)
+    finally:
+        for k, v in old.items():
+            if v is None:
+                del os.environ[k]
+            else:
+                os.environ[k] = v
+
+
+def device_csr(tok, data, doc_off, flags):
+    """b2t_encode_batch_device: the batch already on the GPU, the result left there; copied back to host arrays
+    (ids, offsets or None, word ids or None, row_ptr) to compare"""
+    import ctypes
+    import torch
+    from tokenizers_b200 import _lib
+    d_bytes = torch.from_numpy(np.ascontiguousarray(data, dtype=np.uint8)).cuda()
+    d_off = torch.from_numpy(np.asarray(doc_off).astype(np.int64)).cuda()
+    L = _lib.lib()
+    res = ctypes.c_void_p()
+    _lib.check(L.b2t_encode_batch_device(tok.handle, d_bytes.data_ptr(), int(doc_off[-1]), d_off.data_ptr(), len(doc_off) - 1, flags, None,
+                                         ctypes.byref(res)))
+    try:
+        assert L.b2t_result_on_device(res) == 1
+        T = L.b2t_result_n_tokens(res)
+        cudart = ctypes.CDLL("libcudart.so")
+        torch.cuda.synchronize()
+
+        def dev(ptr, count, dtype):
+            out = np.empty(count, dtype=dtype)
+            if count:
+                assert cudart.cudaMemcpy(ctypes.c_void_p(out.ctypes.data), ctypes.c_void_p(ptr), ctypes.c_size_t(out.nbytes), 2) == 0  # device -> host
+            return out
+        return (dev(L.b2t_result_ids(res), T, np.uint32),
+                dev(L.b2t_result_offsets(res), 2 * T, np.uint32).reshape(-1, 2) if flags & _lib.WANT_OFFSETS else None,
+                dev(L.b2t_result_word_ids(res), T, np.uint32) if flags & _lib.WANT_WORD_IDS else None,
+                dev(L.b2t_result_row_ptr(res), len(doc_off), np.uint64))
+    finally:
+        L.b2t_result_free(res)
+
+
+def host_added_csr(ref, data, doc_off, byte_offsets=False):
+    """What the device extraction (FLAG_ADDED_IDS) must return, from `ref` = oracle_backed_tokenizer(...): the host split
+    (added.py) in front of the oracle, with bit 31 set on the ids of the added tokens found in the text"""
+    from tokenizers_b200 import _lib, added
+    flags = _lib.WANT_OFFSETS | _lib.WANT_WORD_IDS | (_lib.OFFSETS_BYTES if byte_offsets else 0)
+    row_off, parts, cut = added.split_batch(ref._added, data, doc_off)
+    ids, offs, wid, rp = ref._engine_rows(data, row_off, flags)
+    if cut:
+        ids, offs, wid, rp, added_at = added.stitch_rows(data, doc_off, parts, ids, offs, wid, rp, byte_offsets)
+        ids = np.array(ids, dtype=np.uint32)
+        ids[[i for i, _, _ in added_at]] |= np.uint32(1 << 31)
+    return ids, offs, wid, rp
+
+
+# ------------------------------------------------------------------------------------------------- tiled batches
+# Tokenization is per document, so a batch made of copies of one base set of documents, with a short "shim" document of
+# varying length in front of every copy, has an output that is the base set's output repeated (with the shims' in
+# between): the reference runs once per base set and once per distinct shim, not over the whole batch.  The shims move
+# every copy to a different offset relative to the 32 B chunks, 1 KB iterations, 2 KB pages and warp ranges.
+SHIM_TEXT = b"the shim moves the next copy along; "
+
+
+def shim_doc(r):
+    return (SHIM_TEXT * (r // len(SHIM_TEXT) + 1))[:r]
+
+
+def tiled_batch(base_data, base_off, target_bytes, seed=0, shim_max=2048):
+    """-> (data uint8, doc_off uint64, shims): [shim(shims[0]), base..., shim(shims[1]), base..., ...] of at least
+    target_bytes; shim lengths are drawn from 0..shim_max-1"""
+    rng = np.random.default_rng(seed)
+    base_data = np.asarray(base_data, dtype=np.uint8)
+    base_off = np.asarray(base_off, dtype=np.uint64)
+    nb = int(base_off[-1])
+    copies = max(1, -(-int(target_bytes) // (nb + shim_max // 2)))
+    shims = rng.integers(0, shim_max, size=copies).tolist()
+    data = np.empty(sum(shims) + copies * nb, dtype=np.uint8)
+    nd = len(base_off) - 1
+    off = np.empty(copies * (nd + 1) + 1, dtype=np.uint64)
+    pos, k = 0, 0
+    for r in shims:
+        data[pos:pos + r] = np.frombuffer(shim_doc(r), dtype=np.uint8)
+        off[k] = pos
+        pos += r
+        off[k + 1:k + 1 + nd] = base_off[:-1] + np.uint64(pos)
+        data[pos:pos + nb] = base_data
+        pos += nb
+        k += nd + 1
+    off[k] = pos
+    return data, off, shims
+
+
+def tiled_expectation(encode, base_data, base_off, shims):
+    """The output of `encode(data, doc_off) -> (ids, offsets | None, word_ids | None, row_ptr)` for tiled_batch(...),
+    from one call on the base set and one per distinct shim length"""
+    base = encode(np.asarray(base_data, dtype=np.uint8), np.asarray(base_off, dtype=np.uint64))
+    per_shim = {}
+    for r in set(shims):
+        b = np.frombuffer(shim_doc(r), dtype=np.uint8).copy()
+        per_shim[r] = encode(b, np.array([0, r], dtype=np.uint64))
+    parts = [[] for _ in range(3)]
+    counts = []
+    for r in shims:
+        for piece in (per_shim[r], base):
+            for k in range(3):
+                if piece[k] is not None:
+                    parts[k].append(np.asarray(piece[k]))
+            counts.append(np.diff(np.asarray(piece[3], dtype=np.uint64)))
+    out = [np.concatenate(p) if p else None for p in parts]
+    rp = np.zeros(sum(len(c) for c in counts) + 1, dtype=np.uint64)
+    np.cumsum(np.concatenate(counts), out=rp[1:])
+    return out[0], out[1], out[2], rp
+
+
+def k1_kb(n_bytes, sm_count, llama3):
+    """KB of the batch that each warp of the pre-tokenization scan (K1) owns: the formula of launch_pretok in
+    tokenizers_b200/csrc/engine.cu (the lean kernel runs 8 blocks of 4 warps per SM, the Llama-3 kernel 4)"""
+    n_kb = (n_bytes // 32 + 1 + 31) // 32
+    resident = sm_count * (4 if llama3 else 8) * 4
+    kb = -(-n_kb // (4 * resident))
+    return min(128, max(2, (kb + 1) & ~1))
+
+
+def bert_json(flags):
+    """the wordpiece asset behind BertNormalizer(**flags) + BertPreTokenizer: the bert-base pipeline"""
+    js = json.loads(asset_json("wordpiece"))
+    js["normalizer"] = dict(type="BertNormalizer", **flags)
+    js["pre_tokenizer"] = {"type": "BertPreTokenizer"}
+    return json.dumps(js)
+
+
+BERT_UNCASED = dict(clean_text=True, handle_chinese_chars=True, strip_accents=None, lowercase=True)
+
+
+def pipeline_json(name):
+    """tokenizer.json of the pipelines the scale and edge tests run"""
+    if name in ("gpt2_style", "llama3_style", "wordpiece"):
+        return asset_json(name)
+    if name in ("gpt2_noregex", "gpt2_prefix"):
+        j = json.loads(asset_json("gpt2_style"))
+        j["pre_tokenizer"].update({"use_regex": False} if name == "gpt2_noregex" else {"add_prefix_space": True})
+        return json.dumps(j)
+    if name == "bert_uncased":
+        return bert_json(BERT_UNCASED)
+    if name.startswith("added_"):
+        return with_added_tokens(asset_json(name[6:]))
+    raise KeyError(name)
+
+
+def scale_base(name, seed=0, n_corpus=600, n_fuzz=600):
+    """base documents of a tiled batch for pipeline `name`: corpus text and fuzz documents (added-token documents for
+    added_*), packed -> (data, doc_off)"""
+    import corpus
+    from fuzzgen import rand_docs
+    kind = 4 if name in ("wordpiece", "bert_uncased") else 2
+    cd, co = corpus.generate(kind, 300 + seed, 0, n_corpus)
+    docs = corpus.to_strings(cd, co)
+    if name.startswith("added_"):
+        docs += added_token_docs(400 + seed, n_fuzz)
+    elif name == "bert_uncased":   # (fuzz documents may hold the combining-mark order the device refuses)
+        import random
+        rng = random.Random(seed)
+        docs += ["".join(chr(0xAC00 + rng.randrange(11172)) for _ in range(rng.randint(1, 40))) + " 中文x ÀÉÎ" for _ in range(n_fuzz // 4)]
+    else:
+        docs += rand_docs(500 + seed, n_fuzz, max_len=300)
+    return pack_docs(docs)
+
+
 def added_token_docs(seed, n):
     """fuzz documents with the added tokens spliced in: glued to words, surrounded by spaces, back to back, truncated"""
     import random

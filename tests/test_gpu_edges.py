@@ -1,0 +1,199 @@
+"""GPU (-m gpu): probes placed at chosen offsets from the places where the page kernels change code path or run out of
+room, compared with the oracle in full (char and byte offsets).
+
+Edges, relative to a 2 KB page: its start, the end of its first 32 B chunk, +256 B (BPE halo, LONG_PRETOK_MIN), +416 B
+(WordPiece halo: 104 characters of 4 bytes), +1 KB (one K1 iteration); and the 1024-page block of the page and tile
+scans (2 MiB).  Every page holds one probe whose start or end lies at edge + delta.  Two forms: the filler before a
+probe is a document of its own (a document boundary at the probe) or text of the same document (the regex context
+continues into the probe)."""
+import json
+import random
+import numpy as np
+import pytest
+import helpers
+
+pytestmark = pytest.mark.gpu
+
+from tokenizers_b200 import Tokenizer, _lib  # noqa: E402
+from oracle import oracle as orc  # noqa: E402
+
+PAGE = 2048
+EDGES = [0, 32, 256, 416, 1024]
+DELTAS = [-40, -33, -32, -31, -17, -16, -9, -8, -4, -3, -2, -1, 0, 1, 2, 3, 4, 8, 9, 16, 17, 31, 32, 33, 40]
+FILLER = b"lorem ipsum dolor sit amet, consectetur adipiscing elit "
+WIDE = {1: "abcdefghij", 2: "éßжяλ", 3: "中文語あア", 4: "𝒜𝒷𝓬𐐀𐐨"}   # letters (\p{L}) of 1..4 bytes
+
+
+def word(rng, n_bytes, width):
+    """a run of letters of exactly n_bytes, made of `width`-byte characters (ASCII letters first for the remainder)"""
+    r = n_bytes % width
+    return "".join(rng.choice(WIDE[1]) for _ in range(r)) + "".join(rng.choice(WIDE[width]) for _ in range(n_bytes // width))
+
+
+def wordpiece_json(max_chars):
+    """the wordpiece asset with `max_input_chars_per_word` patched and the 4-byte letters of the probes (and their ##
+    forms) added to the vocabulary: a word of them is then [UNK] only because of its length"""
+    j = json.loads(helpers.asset_json("wordpiece"))
+    j["model"]["max_input_chars_per_word"] = max_chars
+    v = j["model"]["vocab"]
+    nxt = max(v.values()) + 1
+    for c in WIDE[4]:
+        for t in (c, "##" + c):
+            v[t], nxt = nxt, nxt + 1
+    return json.dumps(j)
+
+
+def bpe_probes():
+    rng = random.Random(1)
+    out = [word(rng, n, w) for n in (16, 17, 24, 25, 32, 33, 255, 256, 257) for w in (1, 2, 3, 4)]
+    out += [" " * 40 + "x", "\n" * 33 + "x", " \t" * 20, "x" + " " * 33, "x   \n  y"]          # whitespace runs (\s+(?!\S))
+    out += ["don's", "it'S", "we'll", "x''s"]                                              # a contraction split by the edge
+    out += ["1" * n for n in (2, 3, 4, 5, 6, 7, 8, 9, 10)]                                 # Llama-3 digit runs of 3k-1, 3k, 3k+1
+    out += ["!?!...\r\n\r\nx", "--\r\n", ")]}\r\n\r\n\r\n"]                               # punctuation run + \r\n
+    out += ["", "x", "é"]                                                                    # empty and 1-character documents
+    return out
+
+
+def wordpiece_probes(max_chars):
+    rng = random.Random(2)
+    out = []
+    for n in (max_chars - 1, max_chars, max_chars + 1):
+        out += ["".join(rng.choice("abcdefghijklmnop") for _ in range(n)), "".join(rng.choice(WIDE[4]) for _ in range(n))]
+    out += ["a" * max_chars, "𝒜" * max_chars, " " * 40 + "x", "x" + "\t" * 33, "don's", "", "x", "é"]
+    return out
+
+
+BERT_PROBES = ["".join(chr(0xAC00 + (37 * i) % 11172) for i in range(k)) for k in (5, 40, 90)] + ["中文字" * 12, "x中y", "ÀÉÎÕÜ" * 8, "ǅİ"]
+
+
+def place(slots, form, measure=lambda s: len(s.encode("utf-8"))):
+    """slots: [(probe, position, anchor)] with position increasing -> documents: the probe's start ("start") or end
+    ("end") lands at `position`, counted with `measure` (bytes of the batch the kernels see)"""
+    docs, text, pos = [], [], 0
+    for probe, p, anchor in slots:
+        a = p if anchor == "start" else p - measure(probe)
+        gap = a - pos
+        assert gap >= 0, (probe, p, anchor)
+        fill = (FILLER * (gap // len(FILLER) + 1))[:gap].decode()
+        if gap:
+            fill = fill[:-1] + "\n"
+        if form == "doc":
+            docs += [fill, probe]
+        else:
+            text.append(fill + probe)
+            if len(text) == 16:
+                docs.append("".join(text)); text = []
+        pos = a + measure(probe)
+    if text:
+        docs.append("".join(text))
+    return docs
+
+
+def page_slots(probes, deltas=DELTAS):
+    slots, k = [], 1
+    for probe in probes:
+        for e in EDGES:
+            for anchor in ("start", "end"):
+                for d in deltas:
+                    slots.append((probe, k * PAGE + e + d, anchor))
+                    k += 1
+    return slots
+
+
+def scan_block_slots(probes):
+    """around the 2 MiB boundaries of the page and tile scans (1024 pages): one probe per boundary"""
+    rng = random.Random(3)
+    out = []
+    for m, probe in enumerate(probes, start=1):
+        out.append((probe, m * (2 << 20) + rng.choice([-2, -1, 0, 1, 2]), rng.choice(["start", "end"])))
+    return out
+
+
+_exp = {}
+
+
+def check(tj, docs, what, wcache=(True, False), byte_offsets=True):
+    o = orc.Oracle(tj)
+    data, off = helpers.pack_docs(docs)
+    key = (tj, what)
+    if key not in _exp:
+        _exp[key] = (o.encode_batch_csr(data, off), o.encode_batch_csr(data, off, orc.OFF_BYTE) if byte_offsets else None)
+    exp_c, exp_b = _exp[key]
+    for wc in wcache:
+        tok = helpers.tokenizer_with_env(tj, B2T_WCACHE="1" if wc else "0")
+        be = tok.encode_batch_csr(data, off)
+        helpers.assert_csr_equal((be.ids, be.offsets, be.word_ids, be.row_ptr), exp_c, docs, f"{what} wcache={wc}")
+        if exp_b is not None:
+            be = tok.encode_batch_csr(data, off, byte_offsets=True)
+            helpers.assert_csr_equal((be.ids, be.offsets, be.word_ids, be.row_ptr), exp_b, docs, f"{what} byte offsets wcache={wc}")
+
+
+@pytest.mark.parametrize("form", ["doc", "text"])
+@pytest.mark.parametrize("name", ["gpt2_style", "llama3_style"])
+def test_bpe_probes_at_page_edges(name, form):
+    check(helpers.pipeline_json(name), place(page_slots(bpe_probes()), form), f"{name} {form}")
+
+
+@pytest.mark.parametrize("form", ["doc", "text"])
+def test_bpe_probes_without_regex(form):
+    probes = [p for p in bpe_probes() if len(p.encode()) >= 16 or not p]
+    check(helpers.pipeline_json("gpt2_noregex"), place(page_slots(probes, DELTAS[::3]), form), f"noregex {form}", wcache=(True,))
+
+
+@pytest.mark.parametrize("form", ["doc", "text"])
+@pytest.mark.parametrize("max_chars", [100, 104])
+def test_wordpiece_probes_at_page_edges(max_chars, form):
+    check(wordpiece_json(max_chars), place(page_slots(wordpiece_probes(max_chars)), form), f"wordpiece max_chars={max_chars} {form}")
+
+
+@pytest.mark.parametrize("name", ["gpt2_style", "llama3_style", "wordpiece"])
+def test_probes_at_the_scan_block_edge(name):
+    probes = (bpe_probes() if name != "wordpiece" else wordpiece_probes(100))
+    sel = [probes[i] for i in range(0, len(probes), max(1, len(probes) // 8))][:8]
+    for form in ("doc", "text"):
+        check(wordpiece_json(100) if name == "wordpiece" else helpers.pipeline_json(name), place(scan_block_slots(sel), form), f"{name} 2 MiB {form}", wcache=(True,), byte_offsets=False)
+
+
+@pytest.mark.parametrize("coords", ["input", "normalized"])
+def test_bert_expanding_characters_at_page_edges(coords):
+    """Hangul (three jamo with strip_accents), CJK (spaces around it), accents (stripped) straddling page edges of the
+    input or of the normalized batch"""
+    tj = helpers.pipeline_json("bert_uncased")
+    nz = orc.BertNormalizer(**helpers.BERT_UNCASED)
+    measure = (lambda s: len(s.encode("utf-8"))) if coords == "input" else (lambda s: len(nz.normalize(s.encode("utf-8"))[0]))
+    for form in ("doc", "text"):
+        check(tj, place(page_slots(BERT_PROBES, [-9, -3, -2, -1, 0, 1, 2, 3, 9]), form, measure), f"bert {coords} {form}",
+              wcache=(True,), byte_offsets=False)
+
+
+ADDED_SPANS = [(" " * k + "<mask>", "end") for k in (249, 250)] + [("<mask>" + " " * k, "start") for k in (0, 1)] + \
+              [("[SEP2]" + " " * k, "start") for k in (249, 250)] + [(" " * k + "<both>" + " " * k, "start") for k in (124, 125)]
+
+
+def test_added_token_spans_at_page_edges():
+    """spans of 255 / 256 bytes after lstrip / rstrip (ADDED_MAX_SPAN), one starting on a page's last byte; 257 is refused"""
+    tj = helpers.pipeline_json("added_gpt2_style")
+    tok, ref = Tokenizer.from_str(tj), helpers.oracle_backed_tokenizer(tj)
+    assert tok._dev_added
+    for form in ("doc", "text"):
+        slots, k = [], 1
+        for probe, anchor in ADDED_SPANS:
+            for e in (0, 256):
+                for d in (-2, -1, 0, 1, 2):
+                    slots.append(("x" + probe + "y" if form == "text" else probe, k * PAGE + e + d, anchor))
+                    k += 1
+        docs = place(slots, form)
+        data, off = helpers.pack_docs(docs)
+        for byte_offsets in (False, True):
+            exp = helpers.host_added_csr(ref, data, off, byte_offsets)
+            assert np.count_nonzero(exp[0] >> 31) >= len(slots)
+            got = tok._engine_rows(data, off, _lib.WANT_OFFSETS | _lib.WANT_WORD_IDS | _lib.FLAG_ADDED_IDS | (_lib.OFFSETS_BYTES if byte_offsets else 0))
+            helpers.assert_csr_equal(got, exp, docs, f"added spans {form} bytes={byte_offsets}")
+    for over in (" " * 251 + "<mask>", "[SEP2]" + " " * 251, " " * 126 + "<both>" + " " * 125):
+        docs = place([(over, PAGE - 1, "start")], "doc")
+        with pytest.raises(_lib.B2TError) as ei:
+            tok._engine_rows(*helpers.pack_docs(docs), _lib.WANT_OFFSETS | _lib.FLAG_ADDED_IDS)
+        assert ei.value.code == _lib.B2T_ERR_UNSUPPORTED
+        enc = tok.encode_batch(docs, add_special_tokens=False)   # and the tokenizer splits it on the host instead
+        exp = ref.encode_batch(docs, add_special_tokens=False)
+        assert [list(e.ids) for e in enc] == [list(e.ids) for e in exp]
