@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <atomic>
 #include <condition_variable>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -81,9 +82,14 @@ extern "C" int b2t_unicode_class_table(int scheme, uint8_t* out) {
 }
 
 // ------------------------------------------------------------------------------------------------ buffers
+// Device and pinned host buffers own their memory: it is freed with the buffer (after the owner has synchronised).  They
+// are move-only: declaring the move constructor deletes the copies.
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  ~DevBuf() { if (p) cudaFree(p); }
   int ensure(size_t bytes) {
     if (bytes <= cap) return B2T_OK;
     if (p) cudaFree(p);
@@ -93,12 +99,14 @@ struct DevBuf {
     cap = want;
     return B2T_OK;
   }
-  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
   template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 struct PinBuf {
   void* p = nullptr;
   size_t cap = 0;
+  PinBuf() = default;
+  PinBuf(PinBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  ~PinBuf() { if (p) cudaFreeHost(p); }
   int ensure(size_t bytes, bool keep) {
     if (bytes <= cap) return B2T_OK;
     size_t want = bytes + bytes / 4 + 4096;
@@ -108,8 +116,32 @@ struct PinBuf {
     p = q; cap = want;
     return B2T_OK;
   }
-  void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
   template <class T> T* as() const { return reinterpret_cast<T*>(p); }
+};
+
+// Dense mode request (b2t_encode_batch_dense*): the device-side spec plus how L is chosen.
+struct DenseReq {
+  DenseSpec S;
+  bool batch_longest = false;   // padding strategy BatchLongest: L = longest row of the batch (after pad_to_multiple_of)
+  uint32_t multiple = 0;        // pad_to_multiple_of
+  bool want_mask = false;
+};
+
+// How far run_device_pipeline goes: pre-tokenization only (K0..K1b), up to the token count (the caller finishes into its
+// own buffers), or the whole result in the workspace.
+enum RunUntil { RUN_PRETOK, RUN_COUNT, RUN_RESULT };
+
+// The inputs of one pipeline run, kept so that the run can be repeated with a larger long pool.  `dq` (dense mode) points
+// at the caller's request and is only valid during the call.
+struct Request {
+  const uint8_t* bytes = nullptr; int64_t n = 0; const uint64_t* doc_off = nullptr; uint32_t n_docs = 0, flags = 0;
+  RunUntil until = RUN_RESULT; const DenseReq* dq = nullptr;
+};
+
+// The batch the kernels ran on: the request's, or its re-packed (add_prefix_space) or normalized copy in the workspace.
+struct Batch {
+  const uint8_t* bytes = nullptr; int64_t n = 0; const uint64_t* doc_off = nullptr; uint32_t n_docs = 0;
+  const uint32_t* prefix_bits = nullptr;
 };
 
 // Device-side state of one in-flight batch (or chunk).
@@ -117,7 +149,9 @@ struct Workspace {
   DevBuf bytes, doc_off;              // only used by the host path (inputs staged on the device)
   DevBuf doc_bits, start_bits, drop_bits, page_sum, page_carry, block_sum, block_carry, page_first_doc, ctl;
   DevBuf ids, offsets, word_ids, row_ptr, row_ptr_local;
-  const uint64_t* last_doc_off = nullptr; uint32_t last_n_docs = 0, last_flags = 0; int64_t last_n_pages = 0; bool pending = false;  // begin / finish
+  Request req;                        // the last run
+  Batch batch;
+  bool pending = false;               // begin / finish
   DevBuf tmp_ids, tmp_offsets, tmp_word_ids, tile_count, tile_first, tile_lexcl, tile_bsum;  // pass-1 provisional slots + scan
   DevBuf page_long, long_desc, long_desc1, soft_bits, page_soft, lp_id, lp_val, lp_len, lp_plen, lp_aux, lp_out;  // long BPE pre-tokens (long_kernels.cuh)
   unsigned long long pool_cap = 0;
@@ -129,24 +163,12 @@ struct Workspace {
   DevBuf cand0, cand1, cand_any, hard_bits, inner_bits, added_bits, added_head, added_pool;
   uint32_t added_cap = 0;  // added-token extraction (added_kernels.cuh)
   DevBuf pfx_bytes, pfx_doc_off, pfx_local, pfx_block, prefix_bits, pfx_total;  // add_prefix_space re-pack (prefix_kernels.cuh)
-  int64_t n_eff = 0;                  // bytes of the batch the kernels actually ran on (n + inserted spaces)
   cudaStream_t stream = nullptr;
   cudaEvent_t done = nullptr;
   PinBuf h_ctl;                        // total tokens + error flag read back
-  void release() {
-    bytes.release(); doc_off.release(); doc_bits.release(); start_bits.release(); drop_bits.release(); page_sum.release();
-    page_carry.release(); block_sum.release(); block_carry.release(); page_first_doc.release(); ctl.release(); ids.release(); offsets.release();
-    word_ids.release(); row_ptr.release(); row_ptr_local.release(); h_ctl.release();
-    tmp_ids.release(); tmp_offsets.release(); tmp_word_ids.release(); tile_count.release(); tile_first.release(); tile_lexcl.release(); tile_bsum.release();
-    pfx_bytes.release(); pfx_doc_off.release(); pfx_local.release(); pfx_block.release(); prefix_bits.release(); pfx_total.release();
-    dense_ids.release(); dense_mask.release(); dense_len.release();
-    nrm_doc_bits.release(); nrm_pfd.release(); nrm_page_out.release(); nrm_page_chars.release(); nrm_lexcl_o.release(); nrm_bsum_o.release(); nrm_lexcl_c.release();
-    nrm_bsum_c.release(); nrm_tot.release(); nrm_bytes.release(); nrm_src_char.release(); nrm_doc_off.release(); nrm_doc_char0.release();
-    cand0.release(); cand1.release(); cand_any.release(); hard_bits.release(); inner_bits.release(); added_bits.release(); added_head.release(); added_pool.release();
-    wcache.release(); page_long.release(); long_desc.release(); long_desc1.release(); soft_bits.release(); page_soft.release(); lp_id.release(); lp_val.release(); lp_len.release(); lp_plen.release(); lp_aux.release(); lp_out.release();
+  ~Workspace() {                       // (not copyable: the buffers are not)
     if (stream) cudaStreamDestroy(stream);
     if (done) cudaEventDestroy(done);
-    stream = nullptr; done = nullptr;
   }
 };
 
@@ -161,7 +183,6 @@ struct b2t_result {
   uint32_t dense_len = 0;
   const uint32_t* dense_ids = nullptr; const uint8_t* dense_mask = nullptr; const uint32_t* row_len = nullptr;
   PinBuf h_dense_ids, h_dense_mask, h_row_len;
-  void release_host() { h_ids.release(); h_offsets.release(); h_word_ids.release(); h_row_ptr.release(); h_dense_ids.release(); h_dense_mask.release(); h_row_len.release(); }
 };
 
 constexpr int NSLOT = 3;   // chunk workspaces of one host-path call: NSLOT - 1 chunks are in flight while the next is issued
@@ -193,11 +214,11 @@ struct b2t_engine {
   std::condition_variable set_free;
   Workspace dev_ws;          // b2t_encode_batch_device
   struct SlotSet { Workspace slot[NSLOT]; bool busy = false; };
-  std::vector<SlotSet*> sets;   // at most MAX_SLOT_SETS, created on demand
+  std::vector<std::unique_ptr<SlotSet>> sets;   // at most MAX_SLOT_SETS, created on demand
   cudaStream_t own_stream = nullptr;
   size_t chunk_bytes = 64u << 20;
   // pinned result pool
-  std::vector<b2t_result*> pool;
+  std::vector<std::unique_ptr<b2t_result>> pool;
   // profiling
   int profiling = 0;
   int n_rec = 0;
@@ -205,6 +226,10 @@ struct b2t_engine {
   cudaEvent_t rec_ev[MAX_KERNEL_RECORDS + 1];
   bool rec_ev_made = false;
   std::atomic<int> last_launches{0};
+  ~b2t_engine() {   // (b2t_engine_destroy has set the device and synchronised; the buffers free themselves after this)
+    if (rec_ev_made) for (auto& ev : rec_ev) cudaEventDestroy(ev);
+    if (own_stream) cudaStreamDestroy(own_stream);
+  }
 };
 constexpr size_t MAX_SLOT_SETS = 4;
 
@@ -252,7 +277,7 @@ extern "C" int b2t_engine_create(const b2t_config* cfg, b2t_engine** out) {
   if (dev >= ndev) return fail(B2T_ERR_INVALID, "device %d out of range (%d devices)", dev, ndev);
   CU(cudaSetDevice(dev));
 
-  b2t_engine* e = new b2t_engine();
+  std::unique_ptr<b2t_engine, void (*)(b2t_engine*)> e(new b2t_engine(), b2t_engine_destroy);   // destroyed on every error exit
   e->device = dev; e->model = cfg->model; e->pretok = cfg->pretok; e->add_prefix_space = cfg->add_prefix_space;
   cudaDeviceGetAttribute(&e->sm_count, cudaDevAttrMultiProcessorCount, dev);
   if (const char* wc = getenv("B2T_WCACHE")) e->wcache_on = atoi(wc) != 0;
@@ -263,19 +288,15 @@ extern "C" int b2t_engine_create(const b2t_config* cfg, b2t_engine** out) {
   int rc = B2T_OK;
   if ((rc = upload(e->d_cls, ht.cls_packed)) || (rc = upload(e->d_byte_to_id, ht.byte_to_id)) || (rc = upload(e->d_merge, ht.merge_tbl)) ||
       (rc = upload(e->d_word, ht.word_tbl)) || (rc = upload(e->d_pool, ht.word_pool)) || (rc = upload(e->d_edge, ht.edge_tbl)) ||
-      (rc = upload(e->d_tok2, ht.tok2_bits)) || (rc = upload(e->d_tri, ht.tri_bits))) {
-    b2t_engine_destroy(e);
+      (rc = upload(e->d_tok2, ht.tok2_bits)) || (rc = upload(e->d_tri, ht.tri_bits)))
     return rc;
-  }
   if (cfg->bert_normalizer & B2T_NORM_BERT) {
     NormHost nh;
     build_bert_norm((cfg->bert_normalizer & B2T_NORM_CLEAN_TEXT) != 0, (cfg->bert_normalizer & B2T_NORM_CHINESE_CHARS) != 0,
                     (cfg->bert_normalizer & B2T_NORM_STRIP_ACCENTS) != 0, (cfg->bert_normalizer & B2T_NORM_LOWERCASE) != 0, &nh);
-    if (!nh.ok) { b2t_engine_destroy(e); return fail(B2T_ERR_UNSUPPORTED, "BertNormalizer table: an image exceeds three bytes per input byte"); }
-    if ((rc = upload(e->d_nt_blk, nh.blk)) || (rc = upload(e->d_nt_ent, nh.ent)) || (rc = upload(e->d_nt_pool, nh.pool)) || (rc = upload(e->d_nt_ascii, nh.ascii))) {
-      b2t_engine_destroy(e);
+    if (!nh.ok) return fail(B2T_ERR_UNSUPPORTED, "BertNormalizer table: an image exceeds three bytes per input byte");
+    if ((rc = upload(e->d_nt_blk, nh.blk)) || (rc = upload(e->d_nt_ent, nh.ent)) || (rc = upload(e->d_nt_pool, nh.pool)) || (rc = upload(e->d_nt_ascii, nh.ascii)))
       return rc;
-    }
     e->nt.blk = e->d_nt_blk.as<uint16_t>(); e->nt.ent = e->d_nt_ent.as<uint32_t>(); e->nt.pool = e->d_nt_pool.as<uint8_t>(); e->nt.ascii = e->d_nt_ascii.as<uint8_t>();
     e->norm_on = 1;
   }
@@ -299,8 +320,8 @@ extern "C" int b2t_engine_create(const b2t_config* cfg, b2t_engine** out) {
   cudaFuncSetAttribute(model_tile_kernel<MODEL_BPE>, cudaFuncAttributePreferredSharedMemoryCarveout, 86);
   cudaFuncSetAttribute(model_tile_kernel<MODEL_WORDPIECE>, cudaFuncAttributePreferredSharedMemoryCarveout, 86);
   cudaError_t se = cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking);
-  if (se != cudaSuccess) { b2t_engine_destroy(e); return fail(B2T_ERR_CUDA, "cudaStreamCreate failed: %s", cudaGetErrorString(se)); }
-  *out = e;
+  if (se != cudaSuccess) return fail(B2T_ERR_CUDA, "cudaStreamCreate failed: %s", cudaGetErrorString(se));
+  *out = e.release();
   return B2T_OK;
 }
 
@@ -308,14 +329,6 @@ extern "C" void b2t_engine_destroy(b2t_engine* e) {
   if (!e) return;
   cudaSetDevice(e->device);
   cudaDeviceSynchronize();
-  e->dev_ws.release();
-  for (auto* ss : e->sets) { for (auto& s : ss->slot) s.release(); delete ss; }
-  e->d_nt_blk.release(); e->d_nt_ent.release(); e->d_nt_pool.release(); e->d_nt_ascii.release();
-  e->d_at_bytes.release(); e->d_at_off.release(); e->d_at_id.release(); e->d_at_flags.release(); e->d_at_first.release(); e->d_at_pair.release(); e->d_cls_rust.release();
-  e->d_cls.release(); e->d_byte_to_id.release(); e->d_merge.release(); e->d_word.release(); e->d_pool.release(); e->d_edge.release(); e->d_tok2.release(); e->d_tri.release();
-  for (b2t_result* r : e->pool) { r->release_host(); delete r; }
-  if (e->rec_ev_made) for (auto& ev : e->rec_ev) cudaEventDestroy(ev);
-  if (e->own_stream) cudaStreamDestroy(e->own_stream);
   delete e;
 }
 
@@ -383,17 +396,33 @@ static void rec(b2t_engine* e, cudaStream_t st, const char* name) {
   e->n_rec++;
 }
 
-// Dense mode request (b2t_encode_batch_dense*): the device-side spec plus how L is chosen.
-struct DenseReq {
-  DenseSpec S;
-  bool batch_longest = false;   // padding strategy BatchLongest: L = longest row of the batch (after pad_to_multiple_of)
-  uint32_t multiple = 0;        // pad_to_multiple_of
-  bool want_mask = false;
-};
 static uint32_t dense_round(uint32_t len, uint32_t multiple) {
   if (multiple > 0 && len % multiple) len += multiple - len % multiple;
   return len;
 }
+// b2t_dense_spec -> DenseReq, checked
+static int make_dense_req(const b2t_dense_spec* sp, DenseReq* dq) {
+  if (!sp) return fail(B2T_ERR_INVALID, "dense spec is null");
+  if (sp->struct_size != sizeof(b2t_dense_spec)) return fail(B2T_ERR_INVALID, "b2t_dense_spec: struct_size mismatch (%u != %zu)", sp->struct_size, sizeof(b2t_dense_spec));
+  if (sp->n_pre > (uint32_t)DENSE_MAX_SPECIAL || sp->n_post > (uint32_t)DENSE_MAX_SPECIAL)
+    return fail(B2T_ERR_UNSUPPORTED, "templates with more than %d special tokens on one side are not supported", DENSE_MAX_SPECIAL);
+  if ((sp->n_pre && !sp->pre_ids) || (sp->n_post && !sp->post_ids)) return fail(B2T_ERR_INVALID, "dense spec: null special-token list");
+  const uint32_t n_special = sp->n_pre + sp->n_post;
+  // tokenizer/mod.rs:1272-1283: the sequence is truncated to max_length - n_added_tokens
+  if (sp->max_length && sp->max_length < n_special) return fail(B2T_ERR_INVALID, "max_length %u is smaller than the %u special tokens of the template", sp->max_length, n_special);
+  memset(&dq->S, 0, sizeof(dq->S));
+  dq->S.keep_max = sp->max_length ? sp->max_length - n_special : DENSE_NO_LIMIT;
+  dq->S.pad_id = sp->pad_id; dq->S.n_pre = sp->n_pre; dq->S.n_post = sp->n_post;
+  dq->S.trunc_left = sp->truncate_left ? 1 : 0; dq->S.pad_left = sp->pad_left ? 1 : 0;
+  for (uint32_t i = 0; i < sp->n_pre; ++i) dq->S.pre[i] = sp->pre_ids[i];
+  for (uint32_t i = 0; i < sp->n_post; ++i) dq->S.post[i] = sp->post_ids[i];
+  dq->batch_longest = sp->length == 0;
+  dq->multiple = sp->pad_to_multiple_of;
+  dq->S.L = dq->batch_longest ? 0u : dense_round(sp->length, dq->multiple);
+  dq->want_mask = sp->want_mask != 0;
+  return B2T_OK;
+}
+
 // CSR of the workspace -> dense rows in ws.dense_* (asynchronous on st)
 static int launch_dense(b2t_engine* e, Workspace& ws, uint32_t n_docs, const DenseReq& dq, cudaStream_t st) {
   int rc;
@@ -410,18 +439,17 @@ static int launch_dense(b2t_engine* e, Workspace& ws, uint32_t n_docs, const Den
   return B2T_OK;
 }
 
-// Runs K0..K2 for a batch resident on the device.  Does not synchronise.  model_pass=false stops after K1b.
 // pass 2 of the model pass: provisional slots -> CSR at the given destination, row_ptr = token_base + shard-local row_ptr
 static int finish_device(b2t_engine* e, Workspace& ws, uint32_t* d_ids, uint32_t* d_off, uint32_t* d_wid, uint64_t* d_rp,
                          unsigned long long token_base, cudaStream_t st) {
-  const uint32_t flags = ws.last_flags, n_docs = ws.last_n_docs;
-  const int64_t n_pages = ws.last_n_pages;
+  const uint32_t flags = ws.req.flags, n_docs = ws.batch.n_docs;
+  const int64_t n_pages = ws.batch.n / PAGE + 1;
   compact_kernel<<<(unsigned)((n_pages * 32 + 255) / 256), 256, 0, st>>>(
       ws.tile_count.as<uint32_t>(), ws.tile_first.as<uint32_t>(), ws.tile_lexcl.as<unsigned long long>(), ws.tile_bsum.as<unsigned long long>(), n_pages,
       ws.tmp_ids.as<uint32_t>(), (flags & B2T_WANT_OFFSETS) ? ws.tmp_offsets.as<uint2>() : nullptr,
       (flags & B2T_WANT_WORD_IDS) ? ws.tmp_word_ids.as<uint32_t>() : nullptr, d_ids,
       (flags & B2T_WANT_OFFSETS) ? reinterpret_cast<uint2*>(d_off) : nullptr, (flags & B2T_WANT_WORD_IDS) ? d_wid : nullptr);
-  row_ptr_fix_kernel<<<(n_docs + 1 + 255) / 256, 256, 0, st>>>(ws.last_doc_off, n_docs, ws.tile_lexcl.as<unsigned long long>(),
+  row_ptr_fix_kernel<<<(n_docs + 1 + 255) / 256, 256, 0, st>>>(ws.batch.doc_off, n_docs, ws.tile_lexcl.as<unsigned long long>(),
                                                              ws.tile_bsum.as<unsigned long long>(), ws.row_ptr_local.as<uint64_t>(), d_rp, token_base);
   e->last_launches += 2;
   if (ws.norm_active && (flags & B2T_WANT_OFFSETS) && n_docs)
@@ -431,71 +459,89 @@ static int finish_device(b2t_engine* e, Workspace& ws, uint32_t* d_ids, uint32_t
   return B2T_OK;
 }
 
-static int run_device_pipeline(b2t_engine* e, Workspace& ws, const uint8_t* d_bytes, int64_t n, const uint64_t* d_doc_off,
-                               uint32_t n_docs, uint32_t flags, cudaStream_t st, bool model_pass, bool finish = true, const DenseReq* dq = nullptr) {
-  if (n + (int64_t)n_docs >= (1ll << 31)) return fail(B2T_ERR_TOO_LARGE, "batch of %lld bytes exceeds the per-call limit of 2^31-1; split it", (long long)n);
+// bpe_tile on the 1 GB corpus, H100 80GB HBM3 at a 400 W power limit: 2^19 slots 19.7 ms, 2^20 18.6, 2^21 17.4-17.5,
+// 2^22 17.1; 2^21 x 64 B = 128 MiB
+constexpr uint32_t WCACHE_SLOTS = 1u << 21;
+
+// ---- the stages of run_device_pipeline, in the order it calls them
+
+// add_prefix_space: re-pack the batch with the prefix spaces inserted (byte_level.rs:121-125); costs one small host sync
+// for the new size
+static int repack_prefix(b2t_engine* e, Workspace& ws, Batch& b, cudaStream_t st) {
+  if (!e->add_prefix_space || b.n_docs == 0 || b.n == 0) return B2T_OK;
+  const uint8_t* d_bytes = b.bytes; const uint64_t* d_doc_off = b.doc_off; const int64_t n = b.n; const uint32_t n_docs = b.n_docs;
   int rc;
-  const uint32_t* d_prefix_bits = nullptr;
-  if (e->add_prefix_space && n_docs > 0 && n > 0) {
-    // re-pack the batch with the prefix spaces inserted (byte_level.rs:121-125); costs one small host sync for the new size
-    const int64_t cap = n + n_docs + 64;
-    const uint32_t nb = (n_docs + PFX_BLOCK - 1) / PFX_BLOCK;
-    if ((rc = ws.pfx_bytes.ensure(cap)) || (rc = ws.pfx_doc_off.ensure(((size_t)n_docs + 1) * 8)) || (rc = ws.pfx_local.ensure((size_t)n_docs * 4)) ||
-        (rc = ws.pfx_block.ensure((size_t)nb * 4 + 16)) || (rc = ws.prefix_bits.ensure((cap / 32 + 2) * 4)) || (rc = ws.pfx_total.ensure(16)) ||
-        (rc = ws.h_ctl.ensure(sizeof(ctl_block), false)))
-      return rc;
-    CU(cudaMemsetAsync(ws.prefix_bits.p, 0, (cap / 32 + 2) * 4, st));
-    pfx_scan_block_kernel<<<nb, PFX_BLOCK, 0, st>>>(d_bytes, d_doc_off, n_docs, ws.pfx_local.as<uint32_t>(), ws.pfx_block.as<uint32_t>());
-    pfx_scan_top_kernel<<<1, PFX_BLOCK, 0, st>>>(ws.pfx_block.as<uint32_t>(), nb, ws.pfx_total.as<unsigned long long>());
-    pfx_offsets_kernel<<<(n_docs + 1 + 255) / 256, 256, 0, st>>>(d_bytes, d_doc_off, n_docs, ws.pfx_local.as<uint32_t>(), ws.pfx_block.as<uint32_t>(),
-                                                                ws.pfx_total.as<unsigned long long>(), ws.pfx_doc_off.as<uint64_t>(), ws.prefix_bits.as<uint32_t>());
-    pfx_copy_kernel<<<(unsigned)(((int64_t)n_docs * 32 + 255) / 256), 256, 0, st>>>(d_bytes, d_doc_off, ws.pfx_doc_off.as<uint64_t>(), n_docs, ws.pfx_bytes.as<uint8_t>());
-    unsigned long long added = 0;
-    CU(cudaMemcpyAsync(&added, ws.pfx_total.p, 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    d_bytes = ws.pfx_bytes.as<uint8_t>(); d_doc_off = ws.pfx_doc_off.as<uint64_t>(); n += (int64_t)added;
-    d_prefix_bits = ws.prefix_bits.as<uint32_t>();
-  }
+  const int64_t cap = n + n_docs + 64;
+  const uint32_t nb = (n_docs + PFX_BLOCK - 1) / PFX_BLOCK;
+  if ((rc = ws.pfx_bytes.ensure(cap)) || (rc = ws.pfx_doc_off.ensure(((size_t)n_docs + 1) * 8)) || (rc = ws.pfx_local.ensure((size_t)n_docs * 4)) ||
+      (rc = ws.pfx_block.ensure((size_t)nb * 4 + 16)) || (rc = ws.prefix_bits.ensure((cap / 32 + 2) * 4)) || (rc = ws.pfx_total.ensure(16)) ||
+      (rc = ws.h_ctl.ensure(sizeof(ctl_block), false)))
+    return rc;
+  CU(cudaMemsetAsync(ws.prefix_bits.p, 0, (cap / 32 + 2) * 4, st));
+  pfx_scan_block_kernel<<<nb, PFX_BLOCK, 0, st>>>(d_bytes, d_doc_off, n_docs, ws.pfx_local.as<uint32_t>(), ws.pfx_block.as<uint32_t>());
+  pfx_scan_top_kernel<<<1, PFX_BLOCK, 0, st>>>(ws.pfx_block.as<uint32_t>(), nb, ws.pfx_total.as<unsigned long long>());
+  pfx_offsets_kernel<<<(n_docs + 1 + 255) / 256, 256, 0, st>>>(d_bytes, d_doc_off, n_docs, ws.pfx_local.as<uint32_t>(), ws.pfx_block.as<uint32_t>(),
+                                                              ws.pfx_total.as<unsigned long long>(), ws.pfx_doc_off.as<uint64_t>(), ws.prefix_bits.as<uint32_t>());
+  pfx_copy_kernel<<<(unsigned)(((int64_t)n_docs * 32 + 255) / 256), 256, 0, st>>>(d_bytes, d_doc_off, ws.pfx_doc_off.as<uint64_t>(), n_docs, ws.pfx_bytes.as<uint8_t>());
+  unsigned long long added = 0;
+  CU(cudaMemcpyAsync(&added, ws.pfx_total.p, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  b.bytes = ws.pfx_bytes.as<uint8_t>(); b.doc_off = ws.pfx_doc_off.as<uint64_t>(); b.n += (int64_t)added;
+  b.prefix_bits = ws.prefix_bits.as<uint32_t>();
+  return B2T_OK;
+}
+
+// N1-N2 BertNormalizer as a byte-rewriting pre-pass: the kernels after it see the normalized batch, the offsets are mapped
+// back at the end (N3 in finish_device); costs one small host sync for the size of the normalized batch
+static int normalize(b2t_engine* e, Workspace& ws, Batch& b, uint32_t flags, cudaStream_t st) {
   ws.norm_active = false;
-  if (e->norm_on && n > 0 && n_docs > 0) {
-    // BertNormalizer as a byte-rewriting pre-pass: the kernels below see the normalized batch, the offsets are mapped back at the end
-    if (flags & B2T_OFFSETS_BYTES) return fail(B2T_ERR_UNSUPPORTED, "byte offsets are not available behind a normalizer (character offsets are)");
-    const int64_t o_words = n / 32 + 2, o_pages = n / PAGE + 1, o_blk = (o_pages + TSCAN - 1) / TSCAN;
-    if ((rc = ws.nrm_doc_bits.ensure(o_words * 4)) || (rc = ws.nrm_pfd.ensure(o_pages * 4)) || (rc = ws.nrm_page_out.ensure(o_pages * 4)) ||
-        (rc = ws.nrm_page_chars.ensure(o_pages * 4)) || (rc = ws.nrm_lexcl_o.ensure(o_pages * 8)) || (rc = ws.nrm_lexcl_c.ensure(o_pages * 8)) ||
-        (rc = ws.nrm_bsum_o.ensure((o_blk + 2) * 8)) || (rc = ws.nrm_bsum_c.ensure((o_blk + 2) * 8)) || (rc = ws.nrm_tot.ensure(32)) ||
-        (rc = ws.nrm_doc_off.ensure(((size_t)n_docs + 1) * 8)) || (rc = ws.nrm_doc_char0.ensure(((size_t)n_docs + 1) * 4)) || (rc = ws.h_ctl.ensure(sizeof(ctl_block), false)))
-      return rc;
-    CU(cudaMemsetAsync(ws.nrm_doc_bits.p, 0, o_words * 4, st));
-    CU(cudaMemsetAsync(ws.nrm_tot.p, 0, 32, st));
-    rec(e, st, nullptr);
-    unsigned long long* tot = ws.nrm_tot.as<unsigned long long>();
-    uint32_t* nerr = reinterpret_cast<uint32_t*>(tot + 2);
-    doc_mark_kernel<<<(n_docs + 1 + 255) / 256, 256, 0, st>>>(d_doc_off, n_docs, ws.nrm_doc_bits.as<uint32_t>(), ws.nrm_pfd.as<uint32_t>());
-    norm_count_kernel<<<(unsigned)o_pages, NORM_THREADS, 0, st>>>(d_bytes, n, e->nt, ws.nrm_page_out.as<uint32_t>(), ws.nrm_page_chars.as<uint32_t>(), nerr);
-    tile_scan_block_kernel<<<(unsigned)o_blk, TSCAN, 0, st>>>(ws.nrm_page_out.as<uint32_t>(), ws.nrm_lexcl_o.as<unsigned long long>(), ws.nrm_bsum_o.as<unsigned long long>(), o_pages);
-    tile_scan_top_kernel<<<1, TSCAN, 0, st>>>(ws.nrm_bsum_o.as<unsigned long long>(), o_blk, tot);
-    tile_scan_block_kernel<<<(unsigned)o_blk, TSCAN, 0, st>>>(ws.nrm_page_chars.as<uint32_t>(), ws.nrm_lexcl_c.as<unsigned long long>(), ws.nrm_bsum_c.as<unsigned long long>(), o_pages);
-    tile_scan_top_kernel<<<1, TSCAN, 0, st>>>(ws.nrm_bsum_c.as<unsigned long long>(), o_blk, tot + 1);
-    unsigned long long h_tot[3] = {0, 0, 0};
-    CU(cudaMemcpyAsync(h_tot, ws.nrm_tot.p, 24, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));   // one small read: the size of the normalized batch
-    if ((uint32_t)h_tot[2] & ERR_NORM_UNSUPPORTED)
-      return fail(B2T_ERR_UNSUPPORTED, "the text holds a combining character that strip_accents keeps right behind another combining character: "
-                  "their canonical order (NFD) is not restated on the device");
-    const int64_t m = (int64_t)h_tot[0];
-    if (m + (int64_t)n_docs >= (1ll << 31)) return fail(B2T_ERR_TOO_LARGE, "normalized batch of %lld bytes exceeds the per-call limit of 2^31-1; split it", (long long)m);
-    if ((rc = ws.nrm_bytes.ensure((size_t)m + 64)) || (rc = ws.nrm_src_char.ensure(((size_t)m + 1) * 4))) return rc;
-    norm_write_kernel<<<(unsigned)o_pages, NORM_THREADS, 0, st>>>(d_bytes, n, e->nt, ws.nrm_lexcl_o.as<unsigned long long>(), ws.nrm_bsum_o.as<unsigned long long>(),
-                                                               ws.nrm_lexcl_c.as<unsigned long long>(), ws.nrm_bsum_c.as<unsigned long long>(), TSCAN,
-                                                               ws.nrm_pfd.as<uint32_t>(), d_doc_off, n_docs, ws.nrm_bytes.as<uint8_t>(), ws.nrm_src_char.as<uint32_t>(),
-                                                               ws.nrm_doc_off.as<uint64_t>(), ws.nrm_doc_char0.as<uint32_t>(), nerr);
-    CU(cudaGetLastError());
-    rec(e, st, "normalize");
-    d_bytes = ws.nrm_bytes.as<uint8_t>(); d_doc_off = ws.nrm_doc_off.as<uint64_t>(); n = m;
-    ws.norm_active = true;
-  }
-  ws.n_eff = n;
+  if (!e->norm_on || b.n == 0 || b.n_docs == 0) return B2T_OK;
+  const uint8_t* d_bytes = b.bytes; const uint64_t* d_doc_off = b.doc_off; const int64_t n = b.n; const uint32_t n_docs = b.n_docs;
+  int rc;
+  if (flags & B2T_OFFSETS_BYTES) return fail(B2T_ERR_UNSUPPORTED, "byte offsets are not available behind a normalizer (character offsets are)");
+  const int64_t o_words = n / 32 + 2, o_pages = n / PAGE + 1, o_blk = (o_pages + TSCAN - 1) / TSCAN;
+  if ((rc = ws.nrm_doc_bits.ensure(o_words * 4)) || (rc = ws.nrm_pfd.ensure(o_pages * 4)) || (rc = ws.nrm_page_out.ensure(o_pages * 4)) ||
+      (rc = ws.nrm_page_chars.ensure(o_pages * 4)) || (rc = ws.nrm_lexcl_o.ensure(o_pages * 8)) || (rc = ws.nrm_lexcl_c.ensure(o_pages * 8)) ||
+      (rc = ws.nrm_bsum_o.ensure((o_blk + 2) * 8)) || (rc = ws.nrm_bsum_c.ensure((o_blk + 2) * 8)) || (rc = ws.nrm_tot.ensure(32)) ||
+      (rc = ws.nrm_doc_off.ensure(((size_t)n_docs + 1) * 8)) || (rc = ws.nrm_doc_char0.ensure(((size_t)n_docs + 1) * 4)) || (rc = ws.h_ctl.ensure(sizeof(ctl_block), false)))
+    return rc;
+  CU(cudaMemsetAsync(ws.nrm_doc_bits.p, 0, o_words * 4, st));
+  CU(cudaMemsetAsync(ws.nrm_tot.p, 0, 32, st));
+  rec(e, st, nullptr);
+  unsigned long long* tot = ws.nrm_tot.as<unsigned long long>();
+  uint32_t* nerr = reinterpret_cast<uint32_t*>(tot + 2);
+  doc_mark_kernel<<<(n_docs + 1 + 255) / 256, 256, 0, st>>>(d_doc_off, n_docs, ws.nrm_doc_bits.as<uint32_t>(), ws.nrm_pfd.as<uint32_t>());
+  norm_count_kernel<<<(unsigned)o_pages, NORM_THREADS, 0, st>>>(d_bytes, n, e->nt, ws.nrm_page_out.as<uint32_t>(), ws.nrm_page_chars.as<uint32_t>(), nerr);
+  tile_scan_block_kernel<<<(unsigned)o_blk, TSCAN, 0, st>>>(ws.nrm_page_out.as<uint32_t>(), ws.nrm_lexcl_o.as<unsigned long long>(), ws.nrm_bsum_o.as<unsigned long long>(), o_pages);
+  tile_scan_top_kernel<<<1, TSCAN, 0, st>>>(ws.nrm_bsum_o.as<unsigned long long>(), o_blk, tot);
+  tile_scan_block_kernel<<<(unsigned)o_blk, TSCAN, 0, st>>>(ws.nrm_page_chars.as<uint32_t>(), ws.nrm_lexcl_c.as<unsigned long long>(), ws.nrm_bsum_c.as<unsigned long long>(), o_pages);
+  tile_scan_top_kernel<<<1, TSCAN, 0, st>>>(ws.nrm_bsum_c.as<unsigned long long>(), o_blk, tot + 1);
+  e->last_launches += 6;
+  unsigned long long h_tot[3] = {0, 0, 0};
+  CU(cudaMemcpyAsync(h_tot, ws.nrm_tot.p, 24, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));   // one small read: the size of the normalized batch
+  if ((uint32_t)h_tot[2] & ERR_NORM_UNSUPPORTED)
+    return fail(B2T_ERR_UNSUPPORTED, "the text holds a combining character that strip_accents keeps right behind another combining character: "
+                "their canonical order (NFD) is not restated on the device");
+  const int64_t m = (int64_t)h_tot[0];
+  if (m + (int64_t)n_docs >= (1ll << 31)) return fail(B2T_ERR_TOO_LARGE, "normalized batch of %lld bytes exceeds the per-call limit of 2^31-1; split it", (long long)m);
+  if ((rc = ws.nrm_bytes.ensure((size_t)m + 64)) || (rc = ws.nrm_src_char.ensure(((size_t)m + 1) * 4))) return rc;
+  norm_write_kernel<<<(unsigned)o_pages, NORM_THREADS, 0, st>>>(d_bytes, n, e->nt, ws.nrm_lexcl_o.as<unsigned long long>(), ws.nrm_bsum_o.as<unsigned long long>(),
+                                                             ws.nrm_lexcl_c.as<unsigned long long>(), ws.nrm_bsum_c.as<unsigned long long>(), TSCAN,
+                                                             ws.nrm_pfd.as<uint32_t>(), d_doc_off, n_docs, ws.nrm_bytes.as<uint8_t>(), ws.nrm_src_char.as<uint32_t>(),
+                                                             ws.nrm_doc_off.as<uint64_t>(), ws.nrm_doc_char0.as<uint32_t>(), nerr);
+  e->last_launches++;
+  CU(cudaGetLastError());
+  rec(e, st, "normalize");
+  b.bytes = ws.nrm_bytes.as<uint8_t>(); b.doc_off = ws.nrm_doc_off.as<uint64_t>(); b.n = m;
+  ws.norm_active = true;
+  return B2T_OK;
+}
+
+// Sizes the workspace for the batch the kernels run on and clears what they accumulate into.
+static int size_buffers(b2t_engine* e, Workspace& ws, const Batch& b, uint32_t flags, bool model_pass, cudaStream_t st) {
+  const int64_t n = b.n; const uint32_t n_docs = b.n_docs;
+  int rc;
   const int64_t n_words = n / 32 + 2, n_pages = n / PAGE + 1;
   if ((rc = ws.doc_bits.ensure(n_words * 4)) || (rc = ws.start_bits.ensure(n_words * 4)) || (rc = ws.page_sum.ensure(n_pages * 8)) ||
       (rc = ws.page_carry.ensure(n_pages * 8)) || (rc = ws.block_sum.ensure((n_pages / SCAN_BLOCK + 2) * 8)) ||
@@ -504,9 +550,6 @@ static int run_device_pipeline(b2t_engine* e, Workspace& ws, const uint8_t* d_by
     return rc;
   if (pretok_drops_whitespace(e->pretok) && (rc = ws.drop_bits.ensure(n_words * 4))) return rc;
   const bool bpe = e->model == B2T_MODEL_BPE;
-  // bpe_tile on the 1 GB corpus, H100 80GB HBM3 at a 400 W power limit: 2^19 slots 19.7 ms, 2^20 18.6, 2^21 17.4-17.5,
-  // 2^22 17.1; 2^21 x 64 B = 128 MiB
-  constexpr uint32_t WCACHE_SLOTS = 1u << 21;
   if (model_pass && (rc = ws.wcache.ensure((size_t)WCACHE_SLOTS * 64))) return rc;
   if (model_pass && bpe) {
     if ((rc = ws.page_long.ensure(n_pages * 4)) || (rc = ws.long_desc.ensure((size_t)(n / (LONG_PRETOK_MIN + 1) + 2) * sizeof(LongDesc))) ||
@@ -522,7 +565,6 @@ static int run_device_pipeline(b2t_engine* e, Workspace& ws, const uint8_t* d_by
     if ((flags & B2T_WANT_OFFSETS) && ((rc = ws.offsets.ensure((size_t)(n + 1) * 8)) || (rc = ws.tmp_offsets.ensure((size_t)(n + 1) * 8)))) return rc;
     if ((flags & B2T_WANT_WORD_IDS) && ((rc = ws.word_ids.ensure((size_t)(n + 1) * 4)) || (rc = ws.tmp_word_ids.ensure((size_t)(n + 1) * 4)))) return rc;
   }
-  const int64_t n_chunks_all = n / CHUNK + 1;
   if (e->has_added && !(flags & B2T_NO_ADDED_TOKENS)) {
     if (e->add_prefix_space) return fail(B2T_ERR_UNSUPPORTED, "added-token extraction on the device does not combine with add_prefix_space (the prefix goes in front of every piece)");
     if ((rc = ws.cand0.ensure(n_words * 4)) || (rc = ws.cand1.ensure(n_words * 4)) || (rc = ws.cand_any.ensure((n_words / 32 + 2) * 4)) || (rc = ws.hard_bits.ensure(n_words * 4)) ||
@@ -541,11 +583,16 @@ static int run_device_pipeline(b2t_engine* e, Workspace& ws, const uint8_t* d_by
     CU(cudaMemsetAsync(ws.soft_bits.p, 0, n_words * 4, st));
     CU(cudaMemsetAsync(ws.page_soft.p, 0, n_pages, st));
   }
-  e->last_launches = ws.norm_active ? 7 : 0;
+  return B2T_OK;
+}
+
+// K0 doc_mark, [A1-A2 added-token extraction,] K1 pretok_scan, K1b page_scan
+static int scan(b2t_engine* e, Workspace& ws, const Batch& b, bool added, cudaStream_t st) {
+  const uint8_t* d_bytes = b.bytes; const uint64_t* d_doc_off = b.doc_off; const int64_t n = b.n; const uint32_t n_docs = b.n_docs;
+  const int64_t n_words = n / 32 + 2, n_pages = n / PAGE + 1, n_chunks_all = n / CHUNK + 1;
   if (!ws.norm_active) rec(e, st, nullptr);
   doc_mark_kernel<<<(n_docs + 1 + 255) / 256, 256, 0, st>>>(d_doc_off, n_docs, ws.doc_bits.as<uint32_t>(), ws.page_first_doc.as<uint32_t>());
   rec(e, st, "doc_mark"); e->last_launches++;
-  const bool added = e->has_added && !(flags & B2T_NO_ADDED_TOKENS) && n > 0 && n_docs > 0;
   if (added) {
     // added / special tokens (added_vocabulary.rs:430-564): candidates, then one thread per document that holds one
     ctl_block* ctl = ws.ctl.as<ctl_block>();
@@ -569,80 +616,124 @@ static int run_device_pipeline(b2t_engine* e, Workspace& ws, const uint8_t* d_by
                                                                       ws.block_sum.as<uint64_t>(), n_pages);
   page_scan_top_kernel<<<1, SCAN_BLOCK, 0, st>>>(ws.block_sum.as<uint64_t>(), ws.block_carry.as<uint64_t>(), n_scan_blocks);
   rec(e, st, "page_scan"); e->last_launches += 2;
-  if (model_pass && bpe) {
+  return B2T_OK;
+}
+
+// K1c / K2L (BPE): find the long pre-tokens, cut them where no token can span, find the pieces that are still long and
+// merge those into the long pool
+static void long_pretokens(b2t_engine* e, Workspace& ws, const Batch& b, cudaStream_t st) {
+  const uint8_t* d_bytes = b.bytes; const int64_t n = b.n;
+  const int64_t n_pages = n / PAGE + 1;
+  ctl_block* ctl = ws.ctl.as<ctl_block>();
+  LongPool pool;
+  pool.id = ws.lp_id.as<uint32_t>(); pool.val = ws.lp_val.as<uint64_t>(); pool.len = ws.lp_len.as<uint32_t>(); pool.plen = ws.lp_plen.as<uint32_t>();
+  pool.aux = ws.lp_aux.as<uint32_t>(); pool.out = ws.lp_out.as<uint4>(); pool.cap = ws.pool_cap;
+  long_find_kernel<0><<<(unsigned)((n_pages + 7) / 8), 256, 0, st>>>(ws.start_bits.as<uint32_t>(), nullptr, nullptr, n, n_pages, &ctl->lc,
+                                                                    ws.long_desc1.as<LongDesc>(), nullptr, 0ull);
+  soft_cut_kernel<<<(unsigned)(e->sm_count * 4), 256, 0, st>>>(d_bytes, &ctl->lc, ws.long_desc1.as<LongDesc>(), ws.soft_bits.as<uint32_t>(),
+                                                             ws.page_soft.as<uint8_t>(), e->dt);
+  long_find_kernel<1><<<(unsigned)((n_pages + 7) / 8), 256, 0, st>>>(ws.start_bits.as<uint32_t>(), ws.soft_bits.as<uint32_t>(), ws.page_soft.as<uint8_t>(),
+                                                                    n, n_pages, &ctl->lc, ws.long_desc.as<LongDesc>(), ws.page_long.as<int32_t>(), ws.pool_cap);
+  rec(e, st, "long_find"); e->last_launches += 3;
+  bpe_long_kernel<<<(unsigned)(e->sm_count * 2), LONG_THREADS, 0, st>>>(d_bytes, &ctl->lc, ws.long_desc.as<LongDesc>(), pool, e->dt, e->monotone);
+  rec(e, st, "bpe_long"); e->last_launches++;
+}
+
+// K2 model_tile into provisional slots, then pass 2's page token counts -> exclusive scan (the total goes to the control block)
+static void model_and_count(b2t_engine* e, Workspace& ws, const Batch& b, uint32_t flags, bool added, cudaStream_t st) {
+  const int64_t n_pages = b.n / PAGE + 1;
+  ModelParams P;
+  P.bytes = b.bytes; P.n = b.n;
+  P.start_bits = ws.start_bits.as<uint32_t>(); P.drop_bits = ws.drop_bits.as<uint32_t>(); P.doc_bits = ws.doc_bits.as<uint32_t>();
+  P.soft_bits = ws.soft_bits.as<uint32_t>(); P.page_soft = ws.page_soft.as<uint8_t>();
+  P.page_carry = ws.page_carry.as<uint64_t>(); P.block_carry = ws.block_carry.as<uint64_t>(); P.page_first_doc = ws.page_first_doc.as<uint32_t>();
+  P.doc_off = b.doc_off; P.n_docs = b.n_docs;
+  P.flags = ((flags & B2T_WANT_OFFSETS) ? F_OFFSETS : 0u) | ((flags & B2T_WANT_WORD_IDS) ? F_WORD_IDS : 0u) |
+            (((flags & B2T_OFFSETS_BYTES) || ws.norm_active) ? F_BYTE_OFFSETS : 0u);   // behind the normalizer: bytes of the normalized document, mapped back by norm_offsets_kernel
+  P.ids = ws.tmp_ids.as<uint32_t>(); P.offsets = ws.tmp_offsets.as<uint32_t>(); P.word_ids = ws.tmp_word_ids.as<uint32_t>();
+  P.row_ptr = ws.row_ptr_local.as<uint64_t>();
+  P.tile_count = ws.tile_count.as<uint32_t>(); P.tile_first = ws.tile_first.as<uint32_t>();
+  ctl_block* ctl = ws.ctl.as<ctl_block>();
+  P.err_flag = &ctl->err;
+  P.n_tiles = n_pages;
+  P.page_long = ws.page_long.as<int32_t>(); P.long_desc = ws.long_desc.as<LongDesc>(); P.long_out = ws.lp_out.as<uint4>();
+  P.wcache = ws.wcache.as<uint4>(); P.wcache_mask = WCACHE_SLOTS - 1; P.wcache_on = e->wcache_on;
+  P.prefix_bits = b.prefix_bits;
+  P.added_bits = added ? ws.added_bits.as<uint32_t>() : nullptr; P.added_head = ws.added_head.as<uint32_t>(); P.added_pool = ws.added_pool.as<uint2>();
+  P.flag_added = (flags & B2T_FLAG_ADDED_IDS) ? 1u : 0u;
+  P.t = e->dt;
+  if (e->model == B2T_MODEL_BPE) model_tile_kernel<MODEL_BPE><<<(unsigned)n_pages, MODEL_THREADS, 0, st>>>(P);
+  else model_tile_kernel<MODEL_WORDPIECE><<<(unsigned)n_pages, MODEL_THREADS, 0, st>>>(P);
+  rec(e, st, e->model == B2T_MODEL_BPE ? "bpe_tile" : "wordpiece_tile"); e->last_launches++;
+  const int64_t n_tblk = (n_pages + TSCAN - 1) / TSCAN;
+  tile_scan_block_kernel<<<(unsigned)n_tblk, TSCAN, 0, st>>>(ws.tile_count.as<uint32_t>(), ws.tile_lexcl.as<unsigned long long>(),
+                                                           ws.tile_bsum.as<unsigned long long>(), n_pages);
+  tile_scan_top_kernel<<<1, TSCAN, 0, st>>>(ws.tile_bsum.as<unsigned long long>(), n_tblk, &ctl->total);
+  e->last_launches += 2;
+}
+
+// The compaction into the workspace's CSR (unless the caller finishes into its own buffers), then in dense mode the longest
+// row always (the host checks it against L / derives L from it) and the rows themselves now if L is fixed; the control
+// block is queued for the host last
+static int finish_tail(b2t_engine* e, Workspace& ws, cudaStream_t st) {
+  const DenseReq* dq = ws.req.dq;
+  const bool finish = ws.req.until == RUN_RESULT;
+  const uint32_t n_docs = ws.batch.n_docs;
+  int rc;
+  if (finish && (rc = finish_device(e, ws, ws.ids.as<uint32_t>(), ws.offsets.as<uint32_t>(), ws.word_ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), 0ull, st)))
+    return rc;
+  rec(e, st, "scan_compact");
+  if (dq && finish) {
     ctl_block* ctl = ws.ctl.as<ctl_block>();
-    LongPool pool;
-    pool.id = ws.lp_id.as<uint32_t>(); pool.val = ws.lp_val.as<uint64_t>(); pool.len = ws.lp_len.as<uint32_t>(); pool.plen = ws.lp_plen.as<uint32_t>();
-    pool.aux = ws.lp_aux.as<uint32_t>(); pool.out = ws.lp_out.as<uint4>(); pool.cap = ws.pool_cap;
-    // long pre-tokens: find them, cut them where no token can span, find the pieces that are still long
-    long_find_kernel<0><<<(unsigned)((n_pages + 7) / 8), 256, 0, st>>>(ws.start_bits.as<uint32_t>(), nullptr, nullptr, n, n_pages, &ctl->lc,
-                                                                      ws.long_desc1.as<LongDesc>(), nullptr, 0ull);
-    soft_cut_kernel<<<(unsigned)(e->sm_count * 4), 256, 0, st>>>(d_bytes, &ctl->lc, ws.long_desc1.as<LongDesc>(), ws.soft_bits.as<uint32_t>(),
-                                                               ws.page_soft.as<uint8_t>(), e->dt);
-    long_find_kernel<1><<<(unsigned)((n_pages + 7) / 8), 256, 0, st>>>(ws.start_bits.as<uint32_t>(), ws.soft_bits.as<uint32_t>(), ws.page_soft.as<uint8_t>(),
-                                                                      n, n_pages, &ctl->lc, ws.long_desc.as<LongDesc>(), ws.page_long.as<int32_t>(), ws.pool_cap);
-    rec(e, st, "long_find"); e->last_launches += 3;
-    bpe_long_kernel<<<(unsigned)(e->sm_count * 2), LONG_THREADS, 0, st>>>(d_bytes, &ctl->lc, ws.long_desc.as<LongDesc>(), pool, e->dt, e->monotone);
-    rec(e, st, "bpe_long"); e->last_launches++;
+    if (n_docs) row_len_max_kernel<<<(n_docs + 255) / 256, 256, 0, st>>>(ws.row_ptr.as<uint64_t>(), n_docs, dq->S.keep_max, dq->S.n_pre + dq->S.n_post, &ctl->max_row);
+    e->last_launches++;
+    if (!dq->batch_longest && (rc = launch_dense(e, ws, n_docs, *dq, st))) return rc;
+    rec(e, st, "dense_rows");
   }
+  CU(cudaMemcpyAsync(ws.h_ctl.p, ws.ctl.p, sizeof(ctl_block), cudaMemcpyDeviceToHost, st));
+  return B2T_OK;
+}
+
+// Runs ws.req, a batch resident on the device, as far as ws.req.until.  Does not synchronise (except for the small host
+// reads of the prefix re-pack and the normalizer).  The launch count leaves out the prefix re-pack and N3.
+static int run_device_pipeline(b2t_engine* e, Workspace& ws, cudaStream_t st) {
+  const Request& q = ws.req;
+  if (q.n + (int64_t)q.n_docs >= (1ll << 31)) return fail(B2T_ERR_TOO_LARGE, "batch of %lld bytes exceeds the per-call limit of 2^31-1; split it", (long long)q.n);
+  Batch& b = ws.batch;
+  b = Batch{q.bytes, q.n, q.doc_off, q.n_docs, nullptr};
+  e->last_launches = 0;
+  const bool model_pass = q.until != RUN_PRETOK;
+  int rc;
+  if ((rc = repack_prefix(e, ws, b, st)) || (rc = normalize(e, ws, b, q.flags, st)) || (rc = size_buffers(e, ws, b, q.flags, model_pass, st)))
+    return rc;
+  const bool added = e->has_added && !(q.flags & B2T_NO_ADDED_TOKENS) && b.n > 0 && b.n_docs > 0;
+  if ((rc = scan(e, ws, b, added, st))) return rc;
   if (model_pass) {
-    ModelParams P;
-    P.bytes = d_bytes; P.n = n;
-    P.start_bits = ws.start_bits.as<uint32_t>(); P.drop_bits = ws.drop_bits.as<uint32_t>(); P.doc_bits = ws.doc_bits.as<uint32_t>();
-    P.soft_bits = ws.soft_bits.as<uint32_t>(); P.page_soft = ws.page_soft.as<uint8_t>();
-    P.page_carry = ws.page_carry.as<uint64_t>(); P.block_carry = ws.block_carry.as<uint64_t>(); P.page_first_doc = ws.page_first_doc.as<uint32_t>();
-    P.doc_off = d_doc_off; P.n_docs = n_docs;
-    P.flags = ((flags & B2T_WANT_OFFSETS) ? F_OFFSETS : 0u) | ((flags & B2T_WANT_WORD_IDS) ? F_WORD_IDS : 0u) |
-              (((flags & B2T_OFFSETS_BYTES) || ws.norm_active) ? F_BYTE_OFFSETS : 0u);   // behind the normalizer: bytes of the normalized document, mapped back by norm_offsets_kernel
-    P.ids = ws.tmp_ids.as<uint32_t>(); P.offsets = ws.tmp_offsets.as<uint32_t>(); P.word_ids = ws.tmp_word_ids.as<uint32_t>();
-    P.row_ptr = ws.row_ptr_local.as<uint64_t>();
-    P.tile_count = ws.tile_count.as<uint32_t>(); P.tile_first = ws.tile_first.as<uint32_t>();
-    ctl_block* ctl = ws.ctl.as<ctl_block>();
-    P.err_flag = &ctl->err;
-    P.n_tiles = n_pages;
-    P.page_long = ws.page_long.as<int32_t>(); P.long_desc = ws.long_desc.as<LongDesc>(); P.long_out = ws.lp_out.as<uint4>();
-    P.wcache = ws.wcache.as<uint4>(); P.wcache_mask = WCACHE_SLOTS - 1; P.wcache_on = e->wcache_on;
-    P.prefix_bits = d_prefix_bits;
-    P.added_bits = added ? ws.added_bits.as<uint32_t>() : nullptr; P.added_head = ws.added_head.as<uint32_t>(); P.added_pool = ws.added_pool.as<uint2>();
-    P.flag_added = (flags & B2T_FLAG_ADDED_IDS) ? 1u : 0u;
-    P.t = e->dt;
-    if (e->model == B2T_MODEL_BPE) model_tile_kernel<MODEL_BPE><<<(unsigned)n_pages, MODEL_THREADS, 0, st>>>(P);
-    else model_tile_kernel<MODEL_WORDPIECE><<<(unsigned)n_pages, MODEL_THREADS, 0, st>>>(P);
-    rec(e, st, e->model == B2T_MODEL_BPE ? "bpe_tile" : "wordpiece_tile"); e->last_launches++;
-    // pass 2: page token counts -> exclusive scan -> compaction of the provisional slots into the final CSR
-    const int64_t n_tblk = (n_pages + TSCAN - 1) / TSCAN;
-    tile_scan_block_kernel<<<(unsigned)n_tblk, TSCAN, 0, st>>>(ws.tile_count.as<uint32_t>(), ws.tile_lexcl.as<unsigned long long>(),
-                                                             ws.tile_bsum.as<unsigned long long>(), n_pages);
-    tile_scan_top_kernel<<<1, TSCAN, 0, st>>>(ws.tile_bsum.as<unsigned long long>(), n_tblk, &ctl->total);
-    e->last_launches += 2;
-    ws.last_doc_off = d_doc_off; ws.last_n_docs = n_docs; ws.last_flags = flags; ws.last_n_pages = n_pages;
-    if (finish) {
-      if ((rc = finish_device(e, ws, ws.ids.as<uint32_t>(), ws.offsets.as<uint32_t>(), ws.word_ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), 0ull, st))) return rc;
-    }
-    rec(e, st, "scan_compact");
-    if (dq && finish) {
-      // dense mode: the longest row always (the host checks it against L / derives L from it), the rows themselves now if L is fixed
-      ctl_block* ctl = ws.ctl.as<ctl_block>();
-      if (n_docs) row_len_max_kernel<<<(n_docs + 255) / 256, 256, 0, st>>>(ws.row_ptr.as<uint64_t>(), n_docs, dq->S.keep_max, dq->S.n_pre + dq->S.n_post, &ctl->max_row);
-      e->last_launches++;
-      if (!dq->batch_longest && (rc = launch_dense(e, ws, n_docs, *dq, st))) return rc;
-      rec(e, st, "dense_rows");
-    }
-    CU(cudaMemcpyAsync(ws.h_ctl.p, ws.ctl.p, sizeof(ctl_block), cudaMemcpyDeviceToHost, st));
+    if (e->model == B2T_MODEL_BPE) long_pretokens(e, ws, b, st);
+    model_and_count(e, ws, b, q.flags, added, st);
+    if ((rc = finish_tail(e, ws, st))) return rc;
   }
   CU(cudaGetLastError());
   return B2T_OK;
 }
 
-// 0 = ok, -1 = the long pool was too small (grow to *want and rerun), else an error status
-static int check_ctl(const Workspace& ws, unsigned long long* want) {
-  const ctl_block* c = ws.h_ctl.as<ctl_block>();
-  if (c->err & ERR_ADDED_UNSUPPORTED)   // (first: a refused span leaves the later kernels with half of the picture)
-    return fail(B2T_ERR_UNSUPPORTED, "added-token extraction: a span over %d bytes, more spans than one per 16 input bytes, or overlapping spans; "
-                "pass B2T_NO_ADDED_TOKENS and split on the host", ADDED_MAX_SPAN);
-  if ((c->err | c->lc.err) & ERR_INTERNAL) return fail(B2T_ERR_CUDA, "internal error: long pre-token / added-token bookkeeping mismatch");
-  if (c->lc.err & ERR_POOL_OVERFLOW) { *want = c->lc.pool_used; return -1; }
-  return B2T_OK;
+// Checks the control block of a run the host has waited for.  While the long pool was too small (rare: the batch holds
+// more bytes of long pre-tokens than the pool), grows it to what the run asked for and repeats ws.req on st, three runs
+// in all.  *reran tells whether the run was repeated.
+static int check_run(b2t_engine* e, Workspace& ws, cudaStream_t st, bool* reran = nullptr) {
+  for (int attempt = 0;; ++attempt) {
+    const ctl_block* c = ws.h_ctl.as<ctl_block>();
+    if (c->err & ERR_ADDED_UNSUPPORTED)   // (first: a refused span leaves the later kernels with half of the picture)
+      return fail(B2T_ERR_UNSUPPORTED, "added-token extraction: a span over %d bytes, more spans than one per 16 input bytes, or overlapping spans; "
+                  "pass B2T_NO_ADDED_TOKENS and split on the host", ADDED_MAX_SPAN);
+    if ((c->err | c->lc.err) & ERR_INTERNAL) return fail(B2T_ERR_CUDA, "internal error: long pre-token / added-token bookkeeping mismatch");
+    if (!(c->lc.err & ERR_POOL_OVERFLOW)) return B2T_OK;
+    if (attempt >= 2) return fail(B2T_ERR_CUDA, "long pool did not converge");
+    if (reran) *reran = true;
+    int rc;
+    if ((rc = ensure_long_pool(ws, c->lc.pool_used)) || (rc = run_device_pipeline(e, ws, st))) return rc;
+    CU(cudaStreamSynchronize(st));
+  }
 }
 
 static int ensure_events(b2t_engine* e) {
@@ -674,57 +765,52 @@ extern "C" int b2t_engine_last_kernels(const b2t_engine* e, const char** names, 
   return e->last_launches;
 }
 
-extern "C" int b2t_encode_batch_device(b2t_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off,
-                                       uint32_t n_docs, uint32_t flags, void* stream, b2t_result** out) {
-  if (!e || !out || !d_doc_off || (!d_bytes && n_bytes)) return fail(B2T_ERR_INVALID, "b2t_encode_batch_device: null argument");
-  if (((uintptr_t)d_bytes & 15u) != 0) return fail(B2T_ERR_INVALID, "b2t_encode_batch_device: d_bytes must be 16-byte aligned");
+// The device-resident entry points: argument checks (and in dense mode the spec, read into *dq), then the whole call under
+// dev_mu on the engine's one device workspace, on the caller's stream or the engine's own.  `done(ws, st)` takes the
+// finished run after the host has waited for it.
+template <class Done>
+static int device_encode(const char* fn, b2t_engine* e, const void* out, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off,
+                         uint32_t n_docs, uint32_t flags, RunUntil until, const b2t_dense_spec* spec, DenseReq* dq, void* stream, Done&& done) {
+  if (!e || !out || !d_doc_off || (!d_bytes && n_bytes)) return fail(B2T_ERR_INVALID, "%s: null argument", fn);
+  if (((uintptr_t)d_bytes & 15u) != 0) return fail(B2T_ERR_INVALID, "%s: d_bytes must be 16-byte aligned", fn);
+  int rc;
+  if (dq && (rc = make_dense_req(spec, dq))) return rc;
   std::lock_guard<std::mutex> lk(e->dev_mu);
   CU(cudaSetDevice(e->device));
   cudaStream_t st = stream ? (cudaStream_t)stream : e->own_stream;
   Workspace& ws = e->dev_ws;
-  int rc;
-  for (int attempt = 0;; ++attempt) {
-    if ((rc = run_device_pipeline(e, ws, d_bytes, (int64_t)n_bytes, d_doc_off, n_docs, flags, st, true))) return rc;
-    CU(cudaStreamSynchronize(st));
-    unsigned long long want = 0;
-    rc = check_ctl(ws, &want);
-    if (rc == B2T_OK) break;
-    if (rc != -1 || attempt >= 2) return rc == -1 ? fail(B2T_ERR_CUDA, "long pool did not converge") : rc;
-    if ((rc = ensure_long_pool(ws, want))) return rc;  // rare: the batch has more long pre-token bytes than the pool held
-  }
-  b2t_result* r = new b2t_result();
-  r->eng = e; r->on_device = 1; r->n_docs = n_docs;
-  r->n_tokens = ws.h_ctl.as<ctl_block>()->total;
-  r->ids = ws.ids.as<uint32_t>();
-  r->offsets = (flags & B2T_WANT_OFFSETS) ? ws.offsets.as<uint32_t>() : nullptr;
-  r->word_ids = (flags & B2T_WANT_WORD_IDS) ? ws.word_ids.as<uint32_t>() : nullptr;
-  r->row_ptr = ws.row_ptr.as<uint64_t>();
-  *out = r;
-  return B2T_OK;
+  if (until == RUN_COUNT) ws.pending = false;   // (a failed begin leaves nothing to finish)
+  ws.req = Request{d_bytes, (int64_t)n_bytes, d_doc_off, n_docs, flags, until, dq};
+  if ((rc = run_device_pipeline(e, ws, st))) return rc;
+  CU(cudaStreamSynchronize(st));
+  if ((rc = check_run(e, ws, st))) return rc;
+  return done(ws, st);
+}
+
+extern "C" int b2t_encode_batch_device(b2t_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off,
+                                       uint32_t n_docs, uint32_t flags, void* stream, b2t_result** out) {
+  return device_encode("b2t_encode_batch_device", e, out, d_bytes, n_bytes, d_doc_off, n_docs, flags, RUN_RESULT, nullptr, nullptr, stream,
+                       [&](Workspace& ws, cudaStream_t) -> int {
+    b2t_result* r = new b2t_result();
+    r->eng = e; r->on_device = 1; r->n_docs = n_docs;
+    r->n_tokens = ws.h_ctl.as<ctl_block>()->total;
+    r->ids = ws.ids.as<uint32_t>();
+    r->offsets = (flags & B2T_WANT_OFFSETS) ? ws.offsets.as<uint32_t>() : nullptr;
+    r->word_ids = (flags & B2T_WANT_WORD_IDS) ? ws.word_ids.as<uint32_t>() : nullptr;
+    r->row_ptr = ws.row_ptr.as<uint64_t>();
+    *out = r;
+    return B2T_OK;
+  });
 }
 
 extern "C" int b2t_encode_batch_device_begin(b2t_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off,
                                              uint32_t n_docs, uint32_t flags, void* stream, uint64_t* n_tokens) {
-  if (!e || !n_tokens || !d_doc_off || (!d_bytes && n_bytes)) return fail(B2T_ERR_INVALID, "b2t_encode_batch_device_begin: null argument");
-  if (((uintptr_t)d_bytes & 15u) != 0) return fail(B2T_ERR_INVALID, "b2t_encode_batch_device_begin: d_bytes must be 16-byte aligned");
-  std::lock_guard<std::mutex> lk(e->dev_mu);
-  CU(cudaSetDevice(e->device));
-  cudaStream_t st = stream ? (cudaStream_t)stream : e->own_stream;
-  Workspace& ws = e->dev_ws;
-  ws.pending = false;
-  int rc;
-  for (int attempt = 0;; ++attempt) {
-    if ((rc = run_device_pipeline(e, ws, d_bytes, (int64_t)n_bytes, d_doc_off, n_docs, flags, st, true, false))) return rc;
-    CU(cudaStreamSynchronize(st));
-    unsigned long long want = 0;
-    rc = check_ctl(ws, &want);
-    if (rc == B2T_OK) break;
-    if (rc != -1 || attempt >= 2) return rc == -1 ? fail(B2T_ERR_CUDA, "long pool did not converge") : rc;
-    if ((rc = ensure_long_pool(ws, want))) return rc;
-  }
-  *n_tokens = ws.h_ctl.as<ctl_block>()->total;
-  ws.pending = true;
-  return B2T_OK;
+  return device_encode("b2t_encode_batch_device_begin", e, n_tokens, d_bytes, n_bytes, d_doc_off, n_docs, flags, RUN_COUNT, nullptr, nullptr, stream,
+                       [&](Workspace& ws, cudaStream_t) -> int {
+    *n_tokens = ws.h_ctl.as<ctl_block>()->total;
+    ws.pending = true;
+    return B2T_OK;
+  });
 }
 
 extern "C" int b2t_encode_batch_device_finish(b2t_engine* e, uint32_t* d_ids, uint32_t* d_offsets, uint32_t* d_word_ids,
@@ -733,8 +819,8 @@ extern "C" int b2t_encode_batch_device_finish(b2t_engine* e, uint32_t* d_ids, ui
   std::lock_guard<std::mutex> lk(e->dev_mu);
   Workspace& ws = e->dev_ws;
   if (!ws.pending) return fail(B2T_ERR_INVALID, "b2t_encode_batch_device_finish without a matching begin");
-  if ((ws.last_flags & B2T_WANT_OFFSETS) && !d_offsets) return fail(B2T_ERR_INVALID, "offsets were requested at begin: d_offsets is null");
-  if ((ws.last_flags & B2T_WANT_WORD_IDS) && !d_word_ids) return fail(B2T_ERR_INVALID, "word ids were requested at begin: d_word_ids is null");
+  if ((ws.req.flags & B2T_WANT_OFFSETS) && !d_offsets) return fail(B2T_ERR_INVALID, "offsets were requested at begin: d_offsets is null");
+  if ((ws.req.flags & B2T_WANT_WORD_IDS) && !d_word_ids) return fail(B2T_ERR_INVALID, "word ids were requested at begin: d_word_ids is null");
   CU(cudaSetDevice(e->device));
   cudaStream_t st = stream ? (cudaStream_t)stream : e->own_stream;
   ws.pending = false;
@@ -806,78 +892,43 @@ extern "C" int b2t_engine_set_added_tokens(b2t_engine* e, uint32_t n_tokens, con
 }
 
 // ------------------------------------------------------------------------------------------------ dense mode
-static int make_dense_req(const b2t_dense_spec* sp, DenseReq* dq) {
-  if (!sp) return fail(B2T_ERR_INVALID, "dense spec is null");
-  if (sp->struct_size != sizeof(b2t_dense_spec)) return fail(B2T_ERR_INVALID, "b2t_dense_spec: struct_size mismatch (%u != %zu)", sp->struct_size, sizeof(b2t_dense_spec));
-  if (sp->n_pre > (uint32_t)DENSE_MAX_SPECIAL || sp->n_post > (uint32_t)DENSE_MAX_SPECIAL)
-    return fail(B2T_ERR_UNSUPPORTED, "templates with more than %d special tokens on one side are not supported", DENSE_MAX_SPECIAL);
-  if ((sp->n_pre && !sp->pre_ids) || (sp->n_post && !sp->post_ids)) return fail(B2T_ERR_INVALID, "dense spec: null special-token list");
-  const uint32_t n_special = sp->n_pre + sp->n_post;
-  // tokenizer/mod.rs:1272-1283: the sequence is truncated to max_length - n_added_tokens
-  if (sp->max_length && sp->max_length < n_special) return fail(B2T_ERR_INVALID, "max_length %u is smaller than the %u special tokens of the template", sp->max_length, n_special);
-  memset(&dq->S, 0, sizeof(dq->S));
-  dq->S.keep_max = sp->max_length ? sp->max_length - n_special : DENSE_NO_LIMIT;
-  dq->S.pad_id = sp->pad_id; dq->S.n_pre = sp->n_pre; dq->S.n_post = sp->n_post;
-  dq->S.trunc_left = sp->truncate_left ? 1 : 0; dq->S.pad_left = sp->pad_left ? 1 : 0;
-  for (uint32_t i = 0; i < sp->n_pre; ++i) dq->S.pre[i] = sp->pre_ids[i];
-  for (uint32_t i = 0; i < sp->n_post; ++i) dq->S.post[i] = sp->post_ids[i];
-  dq->batch_longest = sp->length == 0;
-  dq->multiple = sp->pad_to_multiple_of;
-  dq->S.L = dq->batch_longest ? 0u : dense_round(sp->length, dq->multiple);
-  dq->want_mask = sp->want_mask != 0;
-  return B2T_OK;
-}
-
 extern "C" int b2t_encode_batch_dense(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, const b2t_dense_spec* spec,
                                       b2t_result** out);
 
 extern "C" int b2t_encode_batch_dense_device(b2t_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off, uint32_t n_docs,
                                              const b2t_dense_spec* spec, void* stream, b2t_result** out) {
-  if (!e || !out || !d_doc_off || (!d_bytes && n_bytes)) return fail(B2T_ERR_INVALID, "b2t_encode_batch_dense_device: null argument");
-  if (((uintptr_t)d_bytes & 15u) != 0) return fail(B2T_ERR_INVALID, "b2t_encode_batch_dense_device: d_bytes must be 16-byte aligned");
   DenseReq dq;
-  int rc;
-  if ((rc = make_dense_req(spec, &dq))) return rc;
-  std::lock_guard<std::mutex> lk(e->dev_mu);
-  CU(cudaSetDevice(e->device));
-  cudaStream_t st = stream ? (cudaStream_t)stream : e->own_stream;
-  Workspace& ws = e->dev_ws;
-  for (int attempt = 0;; ++attempt) {
-    if ((rc = run_device_pipeline(e, ws, d_bytes, (int64_t)n_bytes, d_doc_off, n_docs, 0u, st, true, true, &dq))) return rc;
-    CU(cudaStreamSynchronize(st));
-    unsigned long long want = 0;
-    rc = check_ctl(ws, &want);
-    if (rc == B2T_OK) break;
-    if (rc != -1 || attempt >= 2) return rc == -1 ? fail(B2T_ERR_CUDA, "long pool did not converge") : rc;
-    if ((rc = ensure_long_pool(ws, want))) return rc;
-  }
-  const uint32_t max_row = ws.h_ctl.as<ctl_block>()->max_row;
-  if (dq.batch_longest) {
-    dq.S.L = dense_round(max_row, dq.multiple);
-    if ((rc = launch_dense(e, ws, n_docs, dq, st))) return rc;   // asynchronous on st, like the CSR entry point's result
-  } else if (max_row > dq.S.L) {
-    return fail(B2T_ERR_INVALID, "a row of %u tokens does not fit the dense length %u: enable truncation (the reference returns a longer row here)", max_row, dq.S.L);
-  }
-  b2t_result* r = new b2t_result();
-  r->eng = e; r->on_device = 1; r->n_docs = n_docs;
-  r->n_tokens = ws.h_ctl.as<ctl_block>()->total;
-  r->dense_len = dq.S.L;
-  r->dense_ids = ws.dense_ids.as<uint32_t>(); r->row_len = ws.dense_len.as<uint32_t>();
-  r->dense_mask = dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr;
-  *out = r;
-  return B2T_OK;
+  return device_encode("b2t_encode_batch_dense_device", e, out, d_bytes, n_bytes, d_doc_off, n_docs, 0u, RUN_RESULT, spec, &dq, stream,
+                       [&](Workspace& ws, cudaStream_t st) -> int {
+    int rc2;
+    const uint32_t max_row = ws.h_ctl.as<ctl_block>()->max_row;
+    if (dq.batch_longest) {
+      dq.S.L = dense_round(max_row, dq.multiple);
+      if ((rc2 = launch_dense(e, ws, n_docs, dq, st))) return rc2;   // asynchronous on st, like the CSR entry point's result
+    } else if (max_row > dq.S.L) {
+      return fail(B2T_ERR_INVALID, "a row of %u tokens does not fit the dense length %u: enable truncation (the reference returns a longer row here)", max_row, dq.S.L);
+    }
+    b2t_result* r = new b2t_result();
+    r->eng = e; r->on_device = 1; r->n_docs = n_docs;
+    r->n_tokens = ws.h_ctl.as<ctl_block>()->total;
+    r->dense_len = dq.S.L;
+    r->dense_ids = ws.dense_ids.as<uint32_t>(); r->row_len = ws.dense_len.as<uint32_t>();
+    r->dense_mask = dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr;
+    *out = r;
+    return B2T_OK;
+  });
 }
 
 // ------------------------------------------------------------------------------------------------ host pipeline
 static b2t_result* pool_get(b2t_engine* e) {
   std::lock_guard<std::mutex> lk(e->mu);
-  if (!e->pool.empty()) { b2t_result* r = e->pool.back(); e->pool.pop_back(); return r; }
+  if (!e->pool.empty()) { b2t_result* r = e->pool.back().release(); e->pool.pop_back(); return r; }
   return new b2t_result();
 }
 
 static void pool_put(b2t_engine* e, b2t_result* r) {
   std::lock_guard<std::mutex> lk(e->mu);
-  e->pool.push_back(r);
+  e->pool.emplace_back(r);
 }
 
 // A slot set for one host-path call; blocks while MAX_SLOT_SETS calls are in flight.
@@ -886,9 +937,9 @@ struct SetLease {
   explicit SetLease(b2t_engine* e_) : e(e_), ss(nullptr) {
     std::unique_lock<std::mutex> lk(e->mu);
     while (true) {
-      for (auto* c : e->sets) if (!c->busy) { ss = c; break; }
+      for (auto& c : e->sets) if (!c->busy) { ss = c.get(); break; }
       if (ss) break;
-      if (e->sets.size() < MAX_SLOT_SETS) { ss = new b2t_engine::SlotSet(); e->sets.push_back(ss); break; }
+      if (e->sets.size() < MAX_SLOT_SETS) { e->sets.emplace_back(new b2t_engine::SlotSet()); ss = e->sets.back().get(); break; }
       e->set_free.wait(lk);
     }
     ss->busy = true;
@@ -913,11 +964,19 @@ __global__ void rebase_kernel(uint64_t* doc_off, uint32_t count, uint64_t base) 
 
 struct Chunk { uint32_t d0, d1; uint64_t b0, b1; uint64_t tok_base; };
 
-static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, uint32_t flags, bool pretok_only,
+// Queues the copy of a chunk's dense rows (documents d0 .. d0 + nd - 1) into the pinned result, on the slot's stream.
+static int queue_dense_copy(b2t_result* r, const Workspace& ws, uint32_t d0, uint32_t nd, const DenseReq& dq) {
+  const size_t L = dq.S.L;
+  if (nd && L) {
+    CU(cudaMemcpyAsync(r->h_dense_ids.as<uint32_t>() + (size_t)d0 * L, ws.dense_ids.p, (size_t)nd * L * 4, cudaMemcpyDeviceToHost, ws.stream));
+    if (dq.want_mask) CU(cudaMemcpyAsync(r->h_dense_mask.as<uint8_t>() + (size_t)d0 * L, ws.dense_mask.p, (size_t)nd * L, cudaMemcpyDeviceToHost, ws.stream));
+  }
+  if (nd) CU(cudaMemcpyAsync(r->h_row_len.as<uint32_t>() + d0, ws.dense_len.p, (size_t)nd * 4, cudaMemcpyDeviceToHost, ws.stream));
+  return B2T_OK;
+}
+
+static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, uint32_t flags,
                        b2t_result** out, const DenseReq* dq_in = nullptr) {
-  if (doc_off[0] != 0) return fail(B2T_ERR_INVALID, "doc_off[0] must be 0");
-  for (uint32_t d = 0; d < n_docs; ++d)  // the kernels index the buffer with these: a decreasing offset must never reach them
-    if (doc_off[d + 1] < doc_off[d]) return fail(B2T_ERR_INVALID, "doc_off must be non-decreasing (document %u)", d);
   const uint64_t total_bytes = doc_off[n_docs];
   // ---- split into chunks of whole documents
   std::vector<Chunk> chunks;
@@ -945,13 +1004,13 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
   b2t_result* r = pool_get(e);
   r->eng = e; r->on_device = 0; r->n_docs = n_docs; r->n_tokens = 0;
   int rc;
-  const bool want_off = (flags & B2T_WANT_OFFSETS) || pretok_only, want_wid = (flags & B2T_WANT_WORD_IDS) && !pretok_only;
+  const bool want_off = (flags & B2T_WANT_OFFSETS) != 0, want_wid = (flags & B2T_WANT_WORD_IDS) != 0;
   // initial capacity guess: 0.30 tokens per byte, grown on demand (pinned pool => steady state allocates nothing)
   uint64_t cap_tok = std::max<uint64_t>(total_bytes * 3 / 10 + 1024, 4096);
   if ((rc = r->h_row_ptr.ensure(((size_t)n_docs + 1) * 8, false))) { pool_put(e, r); return rc; }
   auto grow = [&](uint64_t need_tok) -> int {
     int rc2;
-    if (!pretok_only && (rc2 = r->h_ids.ensure(need_tok * 4, true))) return rc2;
+    if ((rc2 = r->h_ids.ensure(need_tok * 4, true))) return rc2;
     if (want_off && (rc2 = r->h_offsets.ensure(need_tok * 8, true))) return rc2;
     if (want_wid && (rc2 = r->h_word_ids.ensure(need_tok * 4, true))) return rc2;
     return B2T_OK;
@@ -970,26 +1029,16 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
 
   uint64_t tok_base = 0;
   const size_t nc = chunks.size();
+  size_t drained = 0;
   // Pipeline over NSLOT device slots: chunk i is issued (H2D + kernels + count read-back) while older chunks compute;
   // drain(i) waits for chunk i's kernels and queues the D2H of its results on the same slot stream.
   auto drain = [&](size_t ci) -> int {
     Chunk& c = chunks[ci];
     Workspace& ws = ss.slot[ci % NSLOT];
     CU(cudaEventSynchronize(ws.done));
-    if (pretok_only) return B2T_OK;
     int rc2;
-    bool reran = false;
-    for (int attempt = 0;; ++attempt) {
-      unsigned long long want = 0;
-      rc2 = check_ctl(ws, &want);
-      if (rc2 == B2T_OK) break;
-      reran = true;
-      if (rc2 != -1 || attempt >= 2) return rc2 == -1 ? fail(B2T_ERR_CUDA, "long pool did not converge") : rc2;
-      // rerun this chunk with a larger pool (its input is still resident in the slot)
-      if ((rc2 = ensure_long_pool(ws, want))) return rc2;
-      if ((rc2 = run_device_pipeline(e, ws, ws.bytes.as<uint8_t>(), (int64_t)(c.b1 - c.b0), ws.doc_off.as<uint64_t>(), c.d1 - c.d0, flags, ws.stream, true, true, dq))) return rc2;
-      CU(cudaStreamSynchronize(ws.stream));
-    }
+    bool reran = false;   // (a rerun finds the chunk's input still resident in the slot)
+    if ((rc2 = check_run(e, ws, ws.stream, &reran))) return rc2;
     const uint64_t nt = ws.h_ctl.as<ctl_block>()->total;
     c.tok_base = tok_base;
     if (dq) {
@@ -1000,14 +1049,8 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
       } else if (max_row > dq->S.L) {
         return fail(B2T_ERR_INVALID, "a row of %u tokens does not fit the dense length %u: enable truncation (the reference returns a longer row here)", max_row, dq->S.L);
       }
-      if (dq->batch_longest || reran) {   // (a fixed length: the rows were queued for the copy right behind the kernels, see below)
-        const size_t L = dq->S.L;
-        if (nd && L) {
-          CU(cudaMemcpyAsync(r->h_dense_ids.as<uint32_t>() + (size_t)c.d0 * L, ws.dense_ids.p, (size_t)nd * L * 4, cudaMemcpyDeviceToHost, ws.stream));
-          if (dq->want_mask) CU(cudaMemcpyAsync(r->h_dense_mask.as<uint8_t>() + (size_t)c.d0 * L, ws.dense_mask.p, (size_t)nd * L, cudaMemcpyDeviceToHost, ws.stream));
-        }
-        if (nd) CU(cudaMemcpyAsync(r->h_row_len.as<uint32_t>() + c.d0, ws.dense_len.p, (size_t)nd * 4, cudaMemcpyDeviceToHost, ws.stream));
-      }
+      // (a fixed length: the rows were queued for the copy right behind the kernels, see issue(); a rerun has replaced them)
+      if ((dq->batch_longest || reran) && (rc2 = queue_dense_copy(r, ws, c.d0, nd, *dq))) return rc2;
       tok_base += nt;
       return B2T_OK;
     }
@@ -1029,47 +1072,37 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     tok_base += nt;
     return B2T_OK;
   };
-  size_t drained = 0;
-  rc = B2T_OK;
-#define CUL(call)                                                                                             \
-  {                                                                                                           \
-    cudaError_t _e = (call);                                                                                  \
-    if (_e != cudaSuccess) { rc = fail(B2T_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__); break; } \
-  }
-  // (a CUDA failure inside the loop must reach the common cleanup below: the pooled result goes back, slot streams are drained)
-  for (size_t ci = 0; ci < nc && rc == B2T_OK; ++ci) {
+  auto issue = [&](size_t ci) -> int {
     Workspace& ws = ss.slot[ci % NSLOT];
-    if ((rc = slot_init(ws))) break;
+    int rc2;
+    if ((rc2 = slot_init(ws))) return rc2;
     if (ci >= NSLOT) {
       // slot reuse: the chunk that used it must be drained and its copies must have landed
-      while (rc == B2T_OK && drained + NSLOT <= ci) rc = drain(drained++);
-      if (rc) break;
-      CUL(cudaStreamSynchronize(ws.stream));
+      while (drained + NSLOT <= ci) if ((rc2 = drain(drained++))) return rc2;
+      CU(cudaStreamSynchronize(ws.stream));
     }
-    Chunk& c = chunks[ci];
+    const Chunk& c = chunks[ci];
     const uint64_t nb = c.b1 - c.b0;
     const uint32_t nd = c.d1 - c.d0;
-    if ((rc = ws.bytes.ensure(nb + 64)) || (rc = ws.doc_off.ensure(((size_t)nd + 1) * 8))) break;
-    if (nb) CUL(cudaMemcpyAsync(ws.bytes.p, bytes + c.b0, nb, cudaMemcpyHostToDevice, ws.stream));
-    CUL(cudaMemcpyAsync(ws.doc_off.p, doc_off + c.d0, ((size_t)nd + 1) * 8, cudaMemcpyHostToDevice, ws.stream));
+    if ((rc2 = ws.bytes.ensure(nb + 64)) || (rc2 = ws.doc_off.ensure(((size_t)nd + 1) * 8))) return rc2;
+    if (nb) CU(cudaMemcpyAsync(ws.bytes.p, bytes + c.b0, nb, cudaMemcpyHostToDevice, ws.stream));
+    CU(cudaMemcpyAsync(ws.doc_off.p, doc_off + c.d0, ((size_t)nd + 1) * 8, cudaMemcpyHostToDevice, ws.stream));
     if (c.b0) rebase_kernel<<<(nd + 1 + 255) / 256, 256, 0, ws.stream>>>(ws.doc_off.as<uint64_t>(), nd + 1, c.b0);
-    rc = run_device_pipeline(e, ws, ws.bytes.as<uint8_t>(), (int64_t)nb, ws.doc_off.as<uint64_t>(), nd, pretok_only ? (flags | B2T_NO_ADDED_TOKENS) : flags, ws.stream, !pretok_only, true, dq);
-    if (rc) break;
-    if (dq && !dq->batch_longest && nd) {
-      // dense rows of a fixed length: their place in the result does not depend on anything the host has to read first, so
-      // the copy back is queued right behind the kernels (the CSR modes need the chunk's token count for that)
-      const size_t L = dq->S.L;
-      if (L) {
-        CUL(cudaMemcpyAsync(r->h_dense_ids.as<uint32_t>() + (size_t)c.d0 * L, ws.dense_ids.p, (size_t)nd * L * 4, cudaMemcpyDeviceToHost, ws.stream));
-        if (dq->want_mask) CUL(cudaMemcpyAsync(r->h_dense_mask.as<uint8_t>() + (size_t)c.d0 * L, ws.dense_mask.p, (size_t)nd * L, cudaMemcpyDeviceToHost, ws.stream));
-      }
-      CUL(cudaMemcpyAsync(r->h_row_len.as<uint32_t>() + c.d0, ws.dense_len.p, (size_t)nd * 4, cudaMemcpyDeviceToHost, ws.stream));
-    }
-    CUL(cudaEventRecord(ws.done, ws.stream));
+    ws.req = Request{ws.bytes.as<uint8_t>(), (int64_t)nb, ws.doc_off.as<uint64_t>(), nd, flags, RUN_RESULT, dq};
+    if ((rc2 = run_device_pipeline(e, ws, ws.stream))) return rc2;
+    // dense rows of a fixed length: their place in the result does not depend on anything the host has to read first, so
+    // the copy back is queued right behind the kernels (the CSR modes need the chunk's token count for that)
+    if (dq && !dq->batch_longest && (rc2 = queue_dense_copy(r, ws, c.d0, nd, *dq))) return rc2;
+    CU(cudaEventRecord(ws.done, ws.stream));
+    return B2T_OK;
+  };
+  // (a failure in either step must reach the common cleanup below: the pooled result goes back, slot streams are drained)
+  rc = B2T_OK;
+  for (size_t ci = 0; ci < nc && rc == B2T_OK; ++ci) {
+    rc = issue(ci);
     // keep at most NSLOT - 1 chunks un-drained so that result copies overlap the next chunks' kernels
     while (rc == B2T_OK && drained + (NSLOT - 1) <= ci) rc = drain(drained++);
   }
-#undef CUL
   while (rc == B2T_OK && drained < nc) rc = drain(drained++);
   for (auto& s : ss.slot) if (s.stream) cudaStreamSynchronize(s.stream);
   if (rc) { pool_put(e, r); return rc; }
@@ -1080,7 +1113,7 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     r->dense_len = dq->S.L;
     r->dense_ids = r->h_dense_ids.as<uint32_t>(); r->row_len = r->h_row_len.as<uint32_t>();
     r->dense_mask = dq->want_mask ? r->h_dense_mask.as<uint8_t>() : nullptr;
-  } else if (!pretok_only) {
+  } else {
     // chunk-relative row_ptr -> batch-relative (host fix-up: one addition per document)
     uint64_t* rp = r->h_row_ptr.as<uint64_t>();
     for (size_t ci = 1; ci < nc; ++ci) {
@@ -1098,48 +1131,49 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
   return B2T_OK;
 }
 
-extern "C" int b2t_encode_batch(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, uint32_t flags,
-                                b2t_result** out) {
-  if (!e || !out || !doc_off || (!bytes && doc_off[n_docs])) return fail(B2T_ERR_INVALID, "b2t_encode_batch: null argument");
+// The host-buffer entry points: argument checks (and in dense mode the spec, read into *dq), then `run(slot set)` on a slot
+// set of the call's own -- and, while per-kernel profiling is on, on the whole engine (the event records are one per engine).
+template <class Run>
+static int host_call(const char* fn, b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, b2t_result** out,
+                     const b2t_dense_spec* spec, DenseReq* dq, Run&& run) {
+  if (!e || !out || !doc_off || (!bytes && doc_off[n_docs])) return fail(B2T_ERR_INVALID, "%s: null argument", fn);
+  int rc;
+  if (dq && (rc = make_dense_req(spec, dq))) return rc;
+  if (doc_off[0] != 0) return fail(B2T_ERR_INVALID, "doc_off[0] must be 0");
+  for (uint32_t d = 0; d < n_docs; ++d)  // the kernels index the buffer with these: a decreasing offset must never reach them
+    if (doc_off[d + 1] < doc_off[d]) return fail(B2T_ERR_INVALID, "doc_off must be non-decreasing (document %u)", d);
   std::unique_lock<std::mutex> prof(e->prof_mu, std::defer_lock);
   SetLease lease(e);
-  if (e->profiling) prof.lock();   // (the per-kernel event records are one per engine)
+  if (e->profiling) prof.lock();
   CU(cudaSetDevice(e->device));
-  return host_encode(e, *lease.ss, bytes, doc_off, n_docs, flags, false, out);
+  return run(*lease.ss);
+}
+
+extern "C" int b2t_encode_batch(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, uint32_t flags,
+                                b2t_result** out) {
+  return host_call("b2t_encode_batch", e, bytes, doc_off, n_docs, out, nullptr, nullptr,
+                   [&](b2t_engine::SlotSet& ss) { return host_encode(e, ss, bytes, doc_off, n_docs, flags, out); });
 }
 
 extern "C" int b2t_encode_batch_dense(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, const b2t_dense_spec* spec,
                                       b2t_result** out) {
-  if (!e || !out || !doc_off || (!bytes && doc_off[n_docs])) return fail(B2T_ERR_INVALID, "b2t_encode_batch_dense: null argument");
   DenseReq dq;
-  int rc;
-  if ((rc = make_dense_req(spec, &dq))) return rc;
-  std::unique_lock<std::mutex> prof(e->prof_mu, std::defer_lock);
-  SetLease lease(e);
-  if (e->profiling) prof.lock();
-  CU(cudaSetDevice(e->device));
-  return host_encode(e, *lease.ss, bytes, doc_off, n_docs, 0u, false, out, &dq);
+  return host_call("b2t_encode_batch_dense", e, bytes, doc_off, n_docs, out, spec, &dq,
+                   [&](b2t_engine::SlotSet& ss) { return host_encode(e, ss, bytes, doc_off, n_docs, 0u, out, &dq); });
 }
 
 // PreTokenizer seam: runs K0/K1 and expands the split bitmaps into (start, end) pairs.  The expansion of the bitmap
 // into the pair list is output formatting and happens on the host (this is an inspection API, not the hot path).
-extern "C" int b2t_pre_tokenize_batch(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, b2t_result** out) {
-  if (!e || !out || !doc_off || (!bytes && doc_off[n_docs])) return fail(B2T_ERR_INVALID, "b2t_pre_tokenize_batch: null argument");
-  std::unique_lock<std::mutex> prof(e->prof_mu, std::defer_lock);
-  SetLease lease(e);
-  if (e->profiling) prof.lock();
-  CU(cudaSetDevice(e->device));
-  if (doc_off[0] != 0) return fail(B2T_ERR_INVALID, "doc_off[0] must be 0");
-  for (uint32_t d = 0; d < n_docs; ++d)  // the kernels index the buffer with these: a decreasing offset must never reach them
-    if (doc_off[d + 1] < doc_off[d]) return fail(B2T_ERR_INVALID, "doc_off must be non-decreasing (document %u)", d);
+static int pre_tokenize(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, b2t_result** out) {
   const uint64_t n = doc_off[n_docs];
-  Workspace& ws = lease.ss->slot[0];
+  Workspace& ws = ss.slot[0];
   int rc;
   if ((rc = slot_init(ws)) || (rc = ws.bytes.ensure(n + 64)) || (rc = ws.doc_off.ensure(((size_t)n_docs + 1) * 8))) return rc;
   if (n) CU(cudaMemcpyAsync(ws.bytes.p, bytes, n, cudaMemcpyHostToDevice, ws.stream));
   CU(cudaMemcpyAsync(ws.doc_off.p, doc_off, ((size_t)n_docs + 1) * 8, cudaMemcpyHostToDevice, ws.stream));
-  if ((rc = run_device_pipeline(e, ws, ws.bytes.as<uint8_t>(), (int64_t)n, ws.doc_off.as<uint64_t>(), n_docs, B2T_NO_ADDED_TOKENS, ws.stream, false))) return rc;  // (a PreTokenizer knows no added tokens)
-  const uint64_t n_eff = (uint64_t)ws.n_eff;
+  ws.req = Request{ws.bytes.as<uint8_t>(), (int64_t)n, ws.doc_off.as<uint64_t>(), n_docs, B2T_NO_ADDED_TOKENS, RUN_PRETOK, nullptr};  // (a PreTokenizer knows no added tokens)
+  if ((rc = run_device_pipeline(e, ws, ws.stream))) return rc;
+  const uint64_t n_eff = (uint64_t)ws.batch.n;   // bytes the kernels ran on (n + inserted prefix spaces)
   const size_t n_words = n_eff / 32 + 2;
   std::vector<uint32_t> sb(n_words), db(n_words, 0u);
   CU(cudaMemcpyAsync(sb.data(), ws.start_bits.p, n_words * 4, cudaMemcpyDeviceToHost, ws.stream));
@@ -1181,6 +1215,11 @@ extern "C" int b2t_pre_tokenize_batch(b2t_engine* e, const uint8_t* bytes, const
   return B2T_OK;
 }
 
+extern "C" int b2t_pre_tokenize_batch(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, b2t_result** out) {
+  return host_call("b2t_pre_tokenize_batch", e, bytes, doc_off, n_docs, out, nullptr, nullptr,
+                   [&](b2t_engine::SlotSet& ss) { return pre_tokenize(e, ss, bytes, doc_off, n_docs, out); });
+}
+
 // ------------------------------------------------------------------------------------------------ results
 extern "C" uint64_t b2t_result_n_tokens(const b2t_result* r) { return r ? r->n_tokens : 0; }
 extern "C" uint32_t b2t_result_n_docs(const b2t_result* r) { return r ? r->n_docs : 0; }
@@ -1198,8 +1237,8 @@ extern "C" void b2t_result_free(b2t_result* r) {
   if (r->on_device || !r->eng) { delete r; return; }
   b2t_engine* e = r->eng;
   std::lock_guard<std::mutex> lk(e->mu);
-  if (e->pool.size() < 4) e->pool.push_back(r);
-  else { cudaSetDevice(e->device); r->release_host(); delete r; }
+  if (e->pool.size() < 4) e->pool.emplace_back(r);
+  else { cudaSetDevice(e->device); delete r; }
 }
 
 extern "C" int b2t_host_alloc(size_t bytes, void** out) {
