@@ -166,6 +166,35 @@ def test_bert_expanding_characters_at_page_edges(coords):
               wcache=(True,), byte_offsets=False)
 
 
+LONG_STARTS = [0, 1000, 2047]   # page offsets of a long word's first byte (a 417-byte split passes the halo only from 2047)
+
+
+def long_word_slots(words):
+    """each word at a document's start, after a space inside a document and at a document's end (the context is part of
+    the probe), with its first byte at each of LONG_STARTS"""
+    slots, k = [], 1
+    for w in words:
+        for ctx in ("{} tail", "head {} tail", "head {}"):
+            for d in LONG_STARTS:
+                slots.append((ctx.format(w), k * PAGE + d - ctx.index("{}"), "start"))
+                k += 2 + len(w.encode()) // PAGE
+    return slots
+
+
+@pytest.mark.parametrize("name", ["gpt2_prefix", "wordpiece", "bert_uncased"])
+def test_long_pretokens_at_document_edges(name):
+    """BPE pre-tokens of more than 256 bytes, whose tokens come from the long pre-pass (with add_prefix_space the
+    inserted space belongs to the one at a document's start), and WordPiece splits longer than the 416-byte halo ([UNK],
+    characters counted past the halo)"""
+    rng = random.Random(4)
+    if name == "gpt2_prefix":
+        words = [word(rng, n, w) for n in (257, 300, 2100) for w in (1, 2, 3)]
+    else:
+        words = [word(rng, n, w) for n in (417, 2100) for w in (1, 2, 4)]
+    tj = wordpiece_json(100) if name == "wordpiece" else helpers.pipeline_json(name)
+    check(tj, place(long_word_slots(words), "doc"), f"long words {name}", byte_offsets=name != "bert_uncased")
+
+
 ADDED_SPANS = [(" " * k + "<mask>", "end") for k in (249, 250)] + [("<mask>" + " " * k, "start") for k in (0, 1)] + \
               [("[SEP2]" + " " * k, "start") for k in (249, 250)] + [(" " * k + "<both>" + " " * k, "start") for k in (124, 125)]
 

@@ -20,6 +20,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 #include "b2t_tables.h"
 #include "added_kernels.cuh"
 #include "long_kernels.cuh"
@@ -117,7 +118,6 @@ constexpr int WC_MAX_BYTES = 24, WC_MAX_TOK = 6, WC_PROBES = 4;
 // rounds are L2-latency bound, not lane bound.
 constexpr int P4_SPLIT_BYTES = 16;
 constexpr int P4_SHORT_G = 8;
-template <int V> struct IntTag { static constexpr int value = V; };
 #define B2T_WC_READY (1ull << 63)
 #define B2T_WC_BUSY (1ull << 62)
 #define B2T_WC_FP ((1ull << 62) - 1ull)
@@ -169,8 +169,14 @@ __device__ __forceinline__ void st_relaxed_v4(uint4* p, uint4 v) {
 }
 constexpr uint32_t WC_LEN_MARK = 0x80000000u;   // bit 31 of the second length word: always set in a written slot
 
+// Looks up the pre-token [s, s + len) unless the cache is off, it is too long or the caller has a reason to `skip` it.
 // Returns true on a hit (tokens written to s_tok).
-__device__ __forceinline__ bool wc_lookup(uint4* cache, uint32_t mask, const WordKey& key, int s, uint32_t* s_tok) {
+__device__ __forceinline__ bool wc_lookup(const ModelParams& P, const uint8_t* s_byte, uint32_t* s_tok, int s, int len, bool skip) {
+  if (!P.wcache_on || len > WC_MAX_BYTES || skip) return false;
+  WordKey key;
+  wc_make_key(s_byte, s, len, key);
+  const uint4* cache = P.wcache;
+  const uint32_t mask = P.wcache_mask;
   uint32_t slot = key.slot & mask;
 #pragma unroll 1
   for (int pr = 0; pr < WC_PROBES; ++pr, slot = (slot + 1) & mask) {
@@ -202,8 +208,14 @@ __device__ __forceinline__ bool wc_lookup(uint4* cache, uint32_t mask, const Wor
   return false;
 }
 
-// Publish the merged pre-token [s, e) (symbols chained by their lengths) into the first free slot of its probe sequence.
-__device__ __forceinline__ void wc_publish(uint4* cache, uint32_t mask, const WordKey& key, int s, int e, const uint32_t* s_tok) {
+// Publish the merged pre-token [s, e) (symbols chained by their lengths) into the first free slot of its probe sequence,
+// under the same conditions as wc_lookup.
+__device__ __forceinline__ void wc_publish(const ModelParams& P, const uint8_t* s_byte, const uint32_t* s_tok, int s, int e, bool skip) {
+  if (!P.wcache_on || e - s > WC_MAX_BYTES || skip) return;
+  WordKey key;
+  wc_make_key(s_byte, s, e - s, key);
+  uint4* const cache = P.wcache;
+  const uint32_t mask = P.wcache_mask;
   uint32_t ids[6] = {0, 0, 0, 0, 0, 0}, lens[6] = {0, 0, 0, 0, 0, 0};
   int nt = 0, p = s;
   while (p < e) {
@@ -330,48 +342,178 @@ __device__ __forceinline__ void coop_bpe(const DeviceTables& t, const uint8_t* s
 }
 
 
-constexpr int MODEL_MINBLOCKS = 8;  // 8 blocks/SM (32 regs, small spills) rather than 5 (48 regs): the kernel is latency-bound
-template <int MODEL>
-__global__ void __launch_bounds__(MODEL_THREADS, MODEL_MINBLOCKS) model_tile_kernel(const ModelParams P) {
-  constexpr int HALO = MODEL == MODEL_BPE ? 256 : 416;
-  constexpr int SPAN = TILE + HALO;
-  constexpr int NW = SPAN / 32;
-  constexpr int TW = TILE / 32;
-  static_assert(NW <= 96, "warp_prefix_words handles <= 96 words");
-  __shared__ __align__(16) uint8_t s_byte[SPAN];
-  __shared__ __align__(16) uint32_t s_tok[SPAN];   // tok_pack(id, length) of the token that starts at each position
-  __shared__ uint32_t s_startb[NW + 1], s_keptb[NW + 1], s_leadb[NW + 1], s_tokb[NW + 1], s_dsb[TW + 1], s_addedb[TW + 1];
-  __shared__ uint16_t s_apref[NW + 1], s_spref[NW + 1], s_lpref[NW + 1], s_tpref[NW + 1];
-  __shared__ int16_t s_dlast[TW + 1];
-  __shared__ uint16_t s_pt[TILE + 2];
-  __shared__ uint16_t s_mq[TILE / THREAD_PATH_MAX + 2];
-  __shared__ uint16_t s_list[SPAN];  // P3/P4: pre-tokens the word cache did not resolve; P7: positions of the tokens
-  uint16_t* const s_miss = s_list;
-  uint16_t* const s_tokpos = s_list;
-  __shared__ int s_nmiss, s_nmiss_hi;  // misses queued from the front (short) and from the back (longer) of s_miss
-  __shared__ int s_tile, s_next, s_nmq, s_P, s_Elast, s_long, s_ntok, s_ntot, s_anysoft;
-  __shared__ unsigned long long s_excl;
-  __shared__ long long s_long_end, s_span_doc_start;
-  __shared__ int s_long_chars;
-  __shared__ int s_nl;                                   // long BPE pre-tokens that start in this page
-  __shared__ uint16_t s_lk[MAX_LONG_PER_PAGE + 1];       // their pre-token indices, in position order
-  __shared__ int s_lcum[MAX_LONG_PER_PAGE + 2];          // exclusive prefix of their token counts
-  __shared__ unsigned long long s_loff[MAX_LONG_PER_PAGE + 1];
+// ------------------------------------------------------------------------------------------------ page state
+// Set bits of `bits` at positions <= x; pref[w] = set bits in the words before w.
+__device__ __forceinline__ int bit_rank_incl(const uint16_t* pref, const uint32_t* bits, int x) {
+  return (int)pref[x >> 5] + __popc(bits[x >> 5] & mask_le(x & 31));
+}
+__device__ __forceinline__ bool bit_at(const uint32_t* bits, int x) { return (bits[x >> 5] >> (x & 31)) & 1u; }
 
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  constexpr int NWARPS = MODEL_THREADS / 32;
-  if (tid == 0) {
-    s_tile = (int)blockIdx.x;
-    s_next = 0; s_nmq = 0; s_long = 0; s_long_chars = 0; s_nl = 0; s_nmiss = 0; s_nmiss_hi = 0; s_anysoft = 0; s_lcum[0] = 0;
+// Shared memory of one page, laid out without padding.  byte / tok: the page + halo and the token starting at each
+// position (tok_pack).  Bitmaps, one bit per position: startb = units of merging (splits of the pre-tokenizer + exact
+// cuts of long ones), keptb = splits the reference keeps (word ids), leadb = first bytes of characters, tokb = token
+// starts, dsb = document starts, addedb = added-token spans; apref / spref / lpref / tpref = exclusive prefix of the
+// popcounts of startb / keptb / leadb / tokb per word.  dlast: last doc start before each word of the page, or -1.
+// pt: the page's pre-token starts, then the end of the last one.  list: pre-tokens the word cache did not resolve, then
+// the positions of the tokens.  BPE: mq = pre-tokens of 33..256 bytes; lk / lcum / loff = the long pre-tokens starting
+// in the page (indices in position order, exclusive prefix of their token counts, place in long_out).
+template <int HALO_>
+struct PageCommon {
+  static constexpr int HALO = HALO_, SPAN = TILE + HALO, NW = SPAN / 32, TW = TILE / 32;
+  static_assert(NW <= 96 && SPAN % 16 == 0, "warp_prefix_words handles <= 96 words; tok is 16-byte aligned");
+  uint8_t byte[SPAN];
+  uint32_t tok[SPAN];
+  long long span_doc_start;  // first byte of the document that spans into this page
+  uint32_t startb[NW + 1], keptb[NW + 1], leadb[NW + 1], tokb[NW + 1], dsb[TW + 1], addedb[TW + 1];
+  uint16_t apref[NW + 1], spref[NW + 1], lpref[NW + 1], tpref[NW + 1];
+  int16_t dlast[TW + 1];
+  uint16_t pt[TILE + 2], list[SPAN];
+  int tile, npt, elast, is_long, ntok, nmiss;
+};
+struct BpePage : PageCommon<256> {
+  uint16_t mq[TILE / THREAD_PATH_MAX + 2], lk[MAX_LONG_PER_PAGE + 1];
+  int nmiss_hi, nmq, anysoft, nl, lcum[MAX_LONG_PER_PAGE + 2];  // nmiss_hi: misses queued from the back of list
+  unsigned long long loff[MAX_LONG_PER_PAGE + 1];
+};
+struct WpPage : PageCommon<416> {
+  long long long_end;  // end of a split that runs past the halo
+  int next, long_chars;
+};
+template <int MODEL> using PageState = std::conditional_t<MODEL == MODEL_BPE, BpePage, WpPage>;
+
+// Tokens of long pre-tokens (resolved by the pre-pass) that precede page position x.  A long WordPiece split is the
+// page's last token.
+__device__ __forceinline__ int long_tokens_before(const BpePage& sh, int x) {
+  int c = 0;
+  for (int a = 0; a < sh.nl; ++a) if ((int)sh.pt[sh.lk[a]] < x) c = sh.lcum[a + 1];
+  return c;
+}
+__device__ __forceinline__ int long_tokens_before(const WpPage&, int) { return 0; }
+
+// [s, e) is a piece of a cut pre-token (not a whole split of the pre-tokenizer): with ignore_merges the whole-word rule
+// and the word cache (whose entries follow that rule) do not apply to it
+__device__ __forceinline__ bool is_piece(const BpePage& sh, int64_t base, int64_t n, int s, int e) {
+  if (!sh.anysoft) return false;
+  const bool real_e = base + e >= n || (e < BpePage::SPAN && bit_at(sh.keptb, e));
+  return !(bit_at(sh.keptb, s) && real_e);
+}
+
+// the pre-token that starts at s (inside the page) is an added token's span: its id comes from the page's list
+template <class S>
+__device__ __forceinline__ bool added_at(const ModelParams& P, const S& sh, int s) { return P.added_bits != nullptr && bit_at(sh.addedb, s); }
+__device__ __forceinline__ uint32_t added_id(const ModelParams& P, int64_t t, int s) {
+  for (uint32_t i = __ldg(P.added_head + t); i != ADDED_NIL;) {
+    const uint2 v = __ldg(P.added_pool + i);
+    if ((int)(v.x & (uint32_t)(PAGE - 1)) == s) return v.x >> 11;
+    i = v.y;
   }
-  __syncthreads();
-  const int64_t t = s_tile;
-  if (t >= P.n_tiles) return;
-  const int64_t base = t * TILE;
-  const int64_t n = P.n;
-  const int64_t n_chunks = n / CHUNK + 1;
+  atomicOr(P.err_flag, ERR_INTERNAL);
+  return 0u;
+}
 
-  // ---------------------------------------------------------------- P0: stage bytes and bitmaps
+// Warp-aggregated append of k, for the lanes with `take`, to the queue q of length *len: one shared atomic per warp.
+// back: the queue grows downwards from q.
+__device__ __forceinline__ void warp_enqueue(uint16_t* q, int* len, bool take, int k, bool back) {
+  const int lane = threadIdx.x & 31;
+  const unsigned m = __ballot_sync(0xFFFFFFFFu, take);
+  int b = 0;
+  if (lane == 0 && m) b = atomicAdd(len, __popc(m));
+  b = __shfl_sync(0xFFFFFFFFu, b, 0) + __popc(m & ((1u << lane) - 1u));
+  if (take) q[back ? -b : b] = (uint16_t)k;
+}
+
+// models/bpe/model.rs:558-567 (ignore_merges): a vocabulary entry is one token.  Called by all 32 lanes (a shuffle):
+// the lane with `ask` looks the pre-token up, every lane learns from lane `leader` whether its group skips the merge.
+__device__ __forceinline__ bool whole_word_gate(const ModelParams& P, const uint8_t* s_byte, uint32_t* s_tok, int s, int e, bool ask, int leader) {
+  if (!P.t.ignore_merges) return false;
+  const int whole = ask && vocab_whole_word(P.t, s_byte, s, e - s, s_tok) ? 1 : 0;
+  return __shfl_sync(0xFFFFFFFFu, whole, leader) != 0;
+}
+
+// g moved by `step` (-1 / +1) to the nearest character boundary of the batch
+__device__ __forceinline__ int64_t char_boundary(const ModelParams& P, int64_t g, int step) {
+  while ((step < 0 ? g > 0 : g < P.n) && (__ldg(P.bytes + g) & 0xC0u) == 0x80u) g += step;
+  return g;
+}
+
+// Where a token's document starts, seen from the page position x where the token's pre-token starts: ds = its first
+// byte, cb = chars of the page before it (negative: it started in an earlier page), wid = the pre-token's word id.
+struct DocOrigin { int64_t ds; int cb; uint32_t wid; };
+template <class S>
+__device__ __forceinline__ DocOrigin doc_origin(const ModelParams& P, const S& sh, int64_t base, int x) {
+  const int xx = x < TILE ? x : TILE - 1;
+  const uint32_t m = sh.dsb[xx >> 5] & mask_le(xx & 31);
+  const int D = m ? (xx & ~31) + 31 - __clz((int)m) : (int)sh.dlast[xx >> 5];  // last doc start at or before x in the page, or -1
+  int2 carry = make_int2(0, 0);
+  if (D < 0) {  // chars / kept splits of the document before this page, counted from its start (pretok_kernels.cuh K1b)
+    const uint64_t c = __ldg(P.page_carry + sh.tile);
+    const uint64_t bc = (c >> 31) & 1ull ? 0ull : __ldg(P.block_carry + (sh.tile >> 10));  // + the scan block's carry
+    carry = make_int2((int)(((uint32_t)c & 0x7FFFFFFFu) + (uint32_t)bc), (int)((uint32_t)(c >> 32) + (uint32_t)(bc >> 32)));
+  }
+  DocOrigin o;
+  o.ds = D >= 0 ? base + D : sh.span_doc_start;
+  o.cb = D >= 0 ? bit_rank_incl(sh.lpref, sh.leadb, D) - 1 : -carry.x;
+  // kept splits before the doc start (the split AT the doc start may itself be removed whitespace)
+  const int wb = D >= 0 ? bit_rank_incl(sh.spref, sh.keptb, D) - (int)bit_at(sh.keptb, D) : -carry.y;
+  o.wid = (uint32_t)(bit_rank_incl(sh.spref, sh.keptb, x) - 1 - wb);
+  return o;
+}
+
+// Offsets and word id of the token in slot `out`: c0 / c1 = chars of the page before its first char / up to its end
+// (for char offsets); g0 / g1 = its bytes in the batch (for byte offsets, widened to whole characters).
+__device__ __forceinline__ void place_token(const ModelParams& P, const DocOrigin& o, unsigned long long out,
+                                            int c0, int c1, int64_t g0, int64_t g1) {
+  if (P.flags & F_OFFSETS) {
+    const bool byte_off = P.flags & F_BYTE_OFFSETS;
+    uint32_t o0, o1;
+    if (!byte_off) {
+      o0 = (uint32_t)(c0 - o.cb); o1 = (uint32_t)(c1 - o.cb);
+    } else {
+      o0 = (uint32_t)(char_boundary(P, g0, -1) - o.ds); o1 = (uint32_t)(char_boundary(P, g1, 1) - o.ds);
+    }
+    if (P.prefix_bits && ((__ldg(P.prefix_bits + (o.ds >> 5)) >> (o.ds & 31)) & 1u)) {
+      // offsets were computed on the document WITH its inserted space: map back (normalizer.rs:503-514)
+      if (o1 == 1u && byte_off) o1 = (uint32_t)(char_boundary(P, o.ds + 2, 1) - o.ds);  // the space alone: its whole first character
+      o0 = o0 ? o0 - 1u : 0u;
+      o1 = o1 > 2u ? o1 - 1u : 1u;
+    }
+    reinterpret_cast<uint2*>(P.offsets)[out] = make_uint2(o0, o1);
+  }
+  if (P.flags & F_WORD_IDS) P.word_ids[out] = o.wid;
+}
+
+// A token of the page logic (and a long WordPiece split's [UNK]) that starts at page position ts: c1 / g1 as above.
+template <class S>
+__device__ __forceinline__ void emit_token(const ModelParams& P, const S& sh, int64_t base, unsigned long long out,
+                                           uint32_t id, int ts, int c1, int64_t g1) {
+  P.ids[out] = (P.flag_added && ts < TILE && added_at(P, sh, ts)) ? (id | 0x80000000u) : id;
+  place_token(P, doc_origin(P, sh, base, ts), out, bit_rank_incl(sh.lpref, sh.leadb, ts) - 1, c1, base + ts, g1);
+}
+
+// ------------------------------------------------------------------------------------------------ page phases
+// The pre-tokens the page logic resolves: pt[0, pproc), whose bytes are [first, eproc).  is_long: the page's last
+// pre-token runs past the halo.  WordPiece: that split is [UNK], emitted on its own.  BPE: long pre-tokens (collected
+// by collect_long_pretokens) are skipped.  Each phase reads it again: with 32 registers, a value live across phases spills.
+struct PageSpan { int first, eproc, pproc; bool is_long, long_kept; };
+template <int MODEL, class S>
+__device__ __forceinline__ PageSpan page_span(const S& sh) {
+  const int Pn = sh.npt;
+  PageSpan r;
+  r.is_long = sh.is_long && Pn > 0;  // without a start in the page the long pre-token belongs to an earlier page
+  const bool wp_long = MODEL == MODEL_WORDPIECE && r.is_long;
+  r.first = Pn ? (int)sh.pt[0] : sh.elast;
+  r.eproc = Pn ? (wp_long ? (int)sh.pt[Pn - 1] : sh.elast) : 0;
+  r.pproc = wp_long ? Pn - 1 : Pn;
+  r.long_kept = wp_long && bit_at(sh.keptb, sh.pt[Pn - 1]);  // WordPiece: the long split is not removed whitespace
+  return r;
+}
+
+// P0-P2: stage bytes and bitmaps, prefix sums, the pre-token starts
+template <int MODEL, class S>
+__device__ __forceinline__ void stage_page(const ModelParams& P, S& sh, int64_t t, int64_t base) {
+  constexpr int SPAN = S::SPAN, NW = S::NW, TW = S::TW;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int64_t n = P.n, n_chunks = n / CHUNK + 1;
   for (int i = tid; i < SPAN / 16; i += MODEL_THREADS) {
     int64_t g = base + (int64_t)i * 16;
     uint4 v = make_uint4(0, 0, 0, 0);
@@ -381,89 +523,87 @@ __global__ void __launch_bounds__(MODEL_THREADS, MODEL_MINBLOCKS) model_tile_ker
       for (int k = 0; k < 16 && g + k < n; ++k) w[k >> 2] |= (uint32_t)__ldg(P.bytes + g + k) << (8 * (k & 3));
       v = make_uint4(w[0], w[1], w[2], w[3]);
     }
-    reinterpret_cast<uint4*>(s_byte)[i] = v;
+    reinterpret_cast<uint4*>(sh.byte)[i] = v;
   }
   for (int w = tid; w <= NW; w += MODEL_THREADS) {
     int64_t gw = base / 32 + w;
     uint32_t sb = (w < NW && gw < n_chunks) ? __ldg(P.start_bits + gw) : 0u;
     uint32_t db = (MODEL == MODEL_WORDPIECE && w < NW && gw < n_chunks) ? __ldg(P.drop_bits + gw) : 0u;
     uint32_t sf = 0u;
-    if (MODEL == MODEL_BPE && w < NW && gw < n_chunks && __ldg(P.page_soft + (gw >> 6))) { sf = __ldg(P.soft_bits + gw); if (sf) s_anysoft = 1; }
-    s_startb[w] = sb | sf;   // where a unit of merging starts: splits of the pre-tokenizer + exact cuts of long ones
-    s_keptb[w] = sb & ~db;   // splits of the pre-tokenizer that the reference keeps (word ids)
-    if (w <= TW) s_dsb[w] = (w < TW && gw < n_chunks) ? __ldg(P.doc_bits + gw) : 0u;
-    if (w <= TW) s_addedb[w] = (P.added_bits && w < TW && gw < n_chunks) ? __ldg(P.added_bits + gw) : 0u;
+    if constexpr (MODEL == MODEL_BPE)
+      if (w < NW && gw < n_chunks && __ldg(P.page_soft + (gw >> 6))) { sf = __ldg(P.soft_bits + gw); if (sf) sh.anysoft = 1; }
+    sh.startb[w] = sb | sf;
+    sh.keptb[w] = sb & ~db;
+    if (w <= TW) sh.dsb[w] = (w < TW && gw < n_chunks) ? __ldg(P.doc_bits + gw) : 0u;
+    if (w <= TW) sh.addedb[w] = (P.added_bits && w < TW && gw < n_chunks) ? __ldg(P.added_bits + gw) : 0u;
   }
   __syncthreads();
   // lead bits (16 bytes per thread: continuation-byte flags by SWAR, two threads make one bitmap word) + symbol init
   static_assert(SPAN / 16 <= MODEL_THREADS && (SPAN / 16) % 2 == 0, "one pass, thread pairs inside a warp");
-  {
-    const int i = tid;
-    const bool act = i < SPAN / 16;
-    const uint4 v = act ? reinterpret_cast<const uint4*>(s_byte)[i] : make_uint4(0u, 0u, 0u, 0u);
-    const uint32_t c0 = v.x & ~(v.x << 1) & 0x80808080u, c1 = v.y & ~(v.y << 1) & 0x80808080u,
-                   c2 = v.z & ~(v.z << 1) & 0x80808080u, c3 = v.w & ~(v.w << 1) & 0x80808080u;   // 10xxxxxx
-    const uint32_t cont = movemask2(c0, c1) | (movemask2(c2, c3) << 8);
-    const int64_t lim = n - base - (int64_t)i * 16;          // valid bytes from this thread's first position on
-    const uint32_t valid = lim >= 16 ? 0xFFFFu : (lim <= 0 ? 0u : ((1u << (int)lim) - 1u));
-    const uint32_t lead16 = ~cont & valid;
-    const uint32_t other = __shfl_down_sync(0xFFFFFFFFu, lead16, 1);
-    if (act && !(i & 1)) s_leadb[i >> 1] = lead16 | (other << 16);
-    if (act) {   // token starts are written by whoever resolves the pre-token
-      uint4* z = reinterpret_cast<uint4*>(s_tok) + 4 * i;
-      z[0] = make_uint4(0u, 0u, 0u, 0u); z[1] = make_uint4(0u, 0u, 0u, 0u); z[2] = make_uint4(0u, 0u, 0u, 0u); z[3] = make_uint4(0u, 0u, 0u, 0u);
-    }
+  const int i = tid;
+  const bool act = i < SPAN / 16;
+  const uint4 v = act ? reinterpret_cast<const uint4*>(sh.byte)[i] : make_uint4(0u, 0u, 0u, 0u);
+  const uint32_t c0 = v.x & ~(v.x << 1) & 0x80808080u, c1 = v.y & ~(v.y << 1) & 0x80808080u,
+                 c2 = v.z & ~(v.z << 1) & 0x80808080u, c3 = v.w & ~(v.w << 1) & 0x80808080u;   // 10xxxxxx
+  const uint32_t cont = movemask2(c0, c1) | (movemask2(c2, c3) << 8);
+  const int64_t lim = n - base - (int64_t)i * 16;          // valid bytes from this thread's first position on
+  const uint32_t valid = lim >= 16 ? 0xFFFFu : (lim <= 0 ? 0u : ((1u << (int)lim) - 1u));
+  const uint32_t lead16 = ~cont & valid;
+  const uint32_t other = __shfl_down_sync(0xFFFFFFFFu, lead16, 1);
+  if (act && !(i & 1)) sh.leadb[i >> 1] = lead16 | (other << 16);
+  if (act) {   // token starts are written by whoever resolves the pre-token
+    uint4* z = reinterpret_cast<uint4*>(sh.tok) + 4 * i;
+    z[0] = make_uint4(0u, 0u, 0u, 0u); z[1] = make_uint4(0u, 0u, 0u, 0u); z[2] = make_uint4(0u, 0u, 0u, 0u); z[3] = make_uint4(0u, 0u, 0u, 0u);
   }
-  if (tid == 0) s_leadb[NW] = 0u;
+  if (tid == 0) sh.leadb[NW] = 0u;
   __syncthreads();
-
-  // ---------------------------------------------------------------- P1/P2: prefixes, end of the last pre-token
+  // prefixes, end of the last pre-token, last doc start before each word, the spanning document's start
   if (warp == 0) {
-    int tot = warp_prefix_words(s_startb, s_apref, TW, lane);  // all starts inside the page
-    if (lane == 0) s_P = tot;
+    int tot = warp_prefix_words(sh.startb, sh.apref, TW, lane);  // all starts inside the page
+    if (lane == 0) sh.npt = tot;
   } else if (warp == 1) {
-    warp_prefix_words(s_keptb, s_spref, NW, lane);
+    warp_prefix_words(sh.keptb, sh.spref, NW, lane);
   } else if (warp == 2) {
-    warp_prefix_words(s_leadb, s_lpref, NW, lane);
+    warp_prefix_words(sh.leadb, sh.lpref, NW, lane);
   } else if (warp == 3) {
     // first start bit at a position >= TILE (the end of the page's last pre-token)
     int found = SPAN;
     for (int w = TW + lane; w < NW; w += 32) {
-      uint32_t b = s_startb[w];
+      uint32_t b = sh.startb[w];
       if (b) { found = w * 32 + (__ffs((int)b) - 1); break; }
     }
 #pragma unroll
     for (int s = 16; s >= 1; s >>= 1) found = min(found, __shfl_xor_sync(0xFFFFFFFFu, found, s));
     int64_t lim = n - base;  // bytes available from the page start
     int is_long = 0;
-    long long long_end = 0;
     if (found >= SPAN) {
       if (lim <= SPAN) found = (int)lim;
       else {
-        // no start inside the halo: the last pre-token is LONG.  Find its true end in the global bitmap.
+        // no start inside the halo: the last pre-token is LONG
         is_long = 1;
-        int64_t gw = (base + SPAN) / 32;
-        long long e = (MODEL == MODEL_BPE) ? n : -1;  // BPE: the pre-pass already knows the end
-        while (e < 0) {
-          int64_t w = gw + lane;
-          uint32_t b = (w < n_chunks) ? __ldg(P.start_bits + w) : 0u;
-          uint32_t any = __ballot_sync(0xFFFFFFFFu, b != 0u);
-          if (any) {
-            int l = __ffs((int)any) - 1;
-            uint32_t bb = __shfl_sync(0xFFFFFFFFu, b, l);
-            e = (gw + l) * 32 + (__ffs((int)bb) - 1);
-          } else if (gw + 32 >= n_chunks) e = n;
-          gw += 32;
-        }
-        long_end = e < n ? e : n;
         found = SPAN;
+        if constexpr (MODEL == MODEL_WORDPIECE) {  // find its true end in the global bitmap (BPE: the pre-pass knows it)
+          int64_t gw = (base + SPAN) / 32;
+          long long e = -1;
+          while (e < 0) {
+            int64_t w = gw + lane;
+            uint32_t b = (w < n_chunks) ? __ldg(P.start_bits + w) : 0u;
+            uint32_t any = __ballot_sync(0xFFFFFFFFu, b != 0u);
+            if (any) {
+              int l = __ffs((int)any) - 1;
+              uint32_t bb = __shfl_sync(0xFFFFFFFFu, b, l);
+              e = (gw + l) * 32 + (__ffs((int)bb) - 1);
+            } else if (gw + 32 >= n_chunks) e = n;
+            gw += 32;
+          }
+          if (lane == 0) sh.long_end = e < n ? e : n;
+        }
       }
     } else if (found > lim) found = (int)lim;
-    if (lane == 0) { s_Elast = found; s_long = is_long; s_long_end = long_end; }
+    if (lane == 0) { sh.elast = found; sh.is_long = is_long; }
   } else if (warp == 4) {
-    // last doc start strictly before each word of the page
-    int mine0 = -1, mine1 = -1;  // lane handles words 2*lane, 2*lane+1
-    uint32_t b0 = s_dsb[2 * lane], b1 = s_dsb[2 * lane + 1];
+    // last doc start strictly before each word of the page; lane handles words 2*lane, 2*lane+1
+    uint32_t b0 = sh.dsb[2 * lane], b1 = sh.dsb[2 * lane + 1];
     int last0 = b0 ? (2 * lane) * 32 + 31 - __clz((int)b0) : -1;
     int last1 = b1 ? (2 * lane + 1) * 32 + 31 - __clz((int)b1) : -1;
     int mx = max(last0, last1), inc = mx;
@@ -474,417 +614,284 @@ __global__ void __launch_bounds__(MODEL_THREADS, MODEL_MINBLOCKS) model_tile_ker
     }
     int before = __shfl_up_sync(0xFFFFFFFFu, inc, 1);
     if (lane == 0) before = -1;
-    mine0 = before; mine1 = max(before, last0);
-    s_dlast[2 * lane] = (int16_t)mine0; s_dlast[2 * lane + 1] = (int16_t)mine1;
-    if (lane == 31) s_dlast[TW] = (int16_t)inc;
+    sh.dlast[2 * lane] = (int16_t)before; sh.dlast[2 * lane + 1] = (int16_t)max(before, last0);
+    if (lane == 31) sh.dlast[TW] = (int16_t)inc;
   } else if (warp == 5 && lane == 0) {
-    // byte position of the start of the document that spans into this page (for byte offsets)
     uint32_t fd = __ldg(P.page_first_doc + t);
-    s_span_doc_start = fd > 0 ? (long long)__ldg(P.doc_off + fd - 1) : 0;
+    sh.span_doc_start = fd > 0 ? (long long)__ldg(P.doc_off + fd - 1) : 0;
   }
   __syncthreads();
-  const int Pn = s_P;
-  const int Elast = s_Elast;
-  const int is_long = s_long && Pn > 0;  // without a start in the page the long pre-token belongs to an earlier page
-  if (tid < TW) {
-    uint32_t bits = s_startb[tid];
-    int idx = s_apref[tid];
-    while (bits) { s_pt[idx++] = (uint16_t)(tid * 32 + __ffs((int)bits) - 1); bits &= bits - 1u; }
+  if (tid < S::TW) {
+    uint32_t bits = sh.startb[tid];
+    int idx = sh.apref[tid];
+    while (bits) { sh.pt[idx++] = (uint16_t)(tid * 32 + __ffs((int)bits) - 1); bits &= bits - 1u; }
   }
-  if (tid == 0) s_pt[Pn] = (uint16_t)Elast;
-  __syncthreads();
-  const int first = Pn ? (int)s_pt[0] : Elast;
-  // WordPiece: a split that does not fit the halo is [UNK] (handled below).  BPE: pre-tokens longer than LONG_PRETOK_MIN were
-  // resolved by the pre-pass; collect them (position order) and blank their bytes so the page logic skips them.
-  const int Eproc = Pn ? ((MODEL == MODEL_WORDPIECE && is_long) ? (int)s_pt[Pn - 1] : Elast) : 0;
-  const int Pproc = (MODEL == MODEL_WORDPIECE && is_long) ? Pn - 1 : Pn;
-  if (MODEL == MODEL_BPE) {
-    int any_long = 0;
-    for (int k = tid; k < Pn; k += MODEL_THREADS)
-      if ((int)s_pt[k + 1] - (int)s_pt[k] > LONG_PRETOK_MIN) { int i = atomicAdd(&s_nl, 1); if (i < MAX_LONG_PER_PAGE) s_lk[i] = (uint16_t)k; any_long = 1; }
-    if (__syncthreads_or(any_long)) {   // (almost every page: no long pre-token, one barrier instead of three)
-    if (tid == 0) {
-      int nl = s_nl;
-      if (nl > MAX_LONG_PER_PAGE) { nl = MAX_LONG_PER_PAGE; atomicOr(P.err_flag, ERR_INTERNAL); }
-      for (int a = 1; a < nl; ++a) { uint16_t v = s_lk[a]; int b = a - 1; while (b >= 0 && s_lk[b] > v) { s_lk[b + 1] = s_lk[b]; --b; } s_lk[b + 1] = v; }
-      const int32_t slot0 = nl ? __ldg(P.page_long + t) : 0;
-      if (nl && slot0 < 0) { atomicOr(P.err_flag, ERR_INTERNAL); nl = 0; }
-      int cum = 0;
-      for (int a = 0; a < nl; ++a) {
-        const LongDesc d = P.long_desc[slot0 + a];
-        if (d.start != base + s_pt[s_lk[a]]) atomicOr(P.err_flag, ERR_INTERNAL);
-        s_lcum[a] = cum; s_loff[a] = d.pool_off;
-        cum += (d.pool_off == ~0ull) ? 0 : (int)d.ntok;
-      }
-      s_lcum[nl] = cum;
-      s_nl = nl;
-    }
-    __syncthreads();
-    for (int a = 0; a < s_nl; ++a) {
-      const int ls = s_pt[s_lk[a]], le = min((int)s_pt[s_lk[a] + 1], SPAN);
-      for (int pos = ls + tid; pos < le; pos += MODEL_THREADS) s_tok[pos] = 0u;
-    }
-    __syncthreads();
-    }
-  }
-  const int n_longs = MODEL == MODEL_BPE ? s_nl : 0;
-  // [s, e) is a piece of a cut pre-token (not a whole split of the pre-tokenizer): with ignore_merges the whole-word rule
-  // and the word cache (whose entries follow that rule) do not apply to it
-  const bool any_soft = MODEL == MODEL_BPE && s_anysoft != 0;
-  auto is_piece = [&](int s, int e) -> bool {
-    if (!any_soft) return false;
-    const bool real_s = (s_keptb[s >> 5] >> (s & 31)) & 1u;
-    const bool real_e = base + e >= n || (e < SPAN && ((s_keptb[e >> 5] >> (e & 31)) & 1u));
-    return !(real_s && real_e);
-  };
-  // number of long-path tokens that precede page position x
-  auto long_tokens_before = [&](int x) -> int {
-    int c = 0;
-    for (int a = 0; a < n_longs; ++a) if ((int)s_pt[s_lk[a]] < x) c = s_lcum[a + 1];
-    return c;
-  };
+  if (tid == 0) sh.pt[sh.npt] = (uint16_t)sh.elast;
+}
 
-  // the pre-token that starts at s (inside the page) is an added token's span: its id comes from the page's list
-  auto added_at = [&](int s) -> bool { return P.added_bits != nullptr && ((s_addedb[s >> 5] >> (s & 31)) & 1u); };
-  auto added_id = [&](int s) -> uint32_t {
-    for (uint32_t i = __ldg(P.added_head + t); i != ADDED_NIL;) {
-      const uint2 v = __ldg(P.added_pool + i);
-      if ((int)(v.x & (uint32_t)(PAGE - 1)) == s) return v.x >> 11;
-      i = v.y;
+// BPE: pre-tokens longer than LONG_PRETOK_MIN were resolved by the pre-pass; collect them (position order) and clear
+// their symbols so that the page logic skips them
+__device__ __forceinline__ void collect_long_pretokens(const ModelParams& P, BpePage& sh, int64_t t, int64_t base) {
+  const int tid = threadIdx.x, Pn = sh.npt;
+  int any_long = 0;
+  for (int k = tid; k < Pn; k += MODEL_THREADS)
+    if ((int)sh.pt[k + 1] - (int)sh.pt[k] > LONG_PRETOK_MIN) { int i = atomicAdd(&sh.nl, 1); if (i < MAX_LONG_PER_PAGE) sh.lk[i] = (uint16_t)k; any_long = 1; }
+  if (!__syncthreads_or(any_long)) return;   // (almost every page: no long pre-token, one barrier instead of three)
+  if (tid == 0) {
+    int nl = sh.nl;
+    if (nl > MAX_LONG_PER_PAGE) { nl = MAX_LONG_PER_PAGE; atomicOr(P.err_flag, ERR_INTERNAL); }
+    for (int a = 1; a < nl; ++a) { uint16_t v = sh.lk[a]; int b = a - 1; while (b >= 0 && sh.lk[b] > v) { sh.lk[b + 1] = sh.lk[b]; --b; } sh.lk[b + 1] = v; }
+    const int32_t slot0 = nl ? __ldg(P.page_long + t) : 0;
+    if (nl && slot0 < 0) { atomicOr(P.err_flag, ERR_INTERNAL); nl = 0; }
+    int cum = 0;
+    for (int a = 0; a < nl; ++a) {
+      const LongDesc d = P.long_desc[slot0 + a];
+      if (d.start != base + sh.pt[sh.lk[a]]) atomicOr(P.err_flag, ERR_INTERNAL);
+      sh.lcum[a] = cum; sh.loff[a] = d.pool_off;
+      cum += (d.pool_off == ~0ull) ? 0 : (int)d.ntok;
     }
-    atomicOr(P.err_flag, ERR_INTERNAL);
-    return 0u;
-  };
-  if (MODEL == MODEL_BPE) {
-    // -------------------------------------------------------------- P3: word cache, one pre-token per thread
-    // (static assignment: a lookup costs the same for every lane, so the warp stays converged)
-    for (int k0 = 0; k0 < Pproc; k0 += MODEL_THREADS) {
-      const int k = k0 + tid;
-      int kind = 0;  // 0 = resolved / nothing to do, 1 = miss (<= 32 bytes), 2 = medium (33..256 bytes)
-      if (k < Pproc) {
-        const int s = s_pt[k], e = s_pt[k + 1], len = e - s;
-        if (added_at(s)) { s_tok[s] = tok_pack(added_id(s), len); kind = 0; }   // an added token: one token, whatever the model says
-        else if (len > LONG_PRETOK_MIN) kind = 0;  // resolved by the pre-pass
-        else if (len > THREAD_PATH_MAX) kind = 2;
-        else {
-          bool hit = false;
-          if (P.wcache_on && len <= WC_MAX_BYTES && !(P.t.ignore_merges && is_piece(s, e))) {
-            WordKey key;
-            wc_make_key(s_byte, s, len, key);
-            hit = wc_lookup(P.wcache, P.wcache_mask, key, s, s_tok);
+    sh.lcum[nl] = cum;
+    sh.nl = nl;
+  }
+  __syncthreads();
+  for (int a = 0; a < sh.nl; ++a) {
+    const int ls = sh.pt[sh.lk[a]], le = min((int)sh.pt[sh.lk[a] + 1], BpePage::SPAN);
+    for (int pos = ls + tid; pos < le; pos += MODEL_THREADS) sh.tok[pos] = 0u;
+  }
+  __syncthreads();
+}
+
+// G lanes x J positions merge the misses [0, count) of the queue; the queue from the back of list when `back`.  count
+// is read from shared memory each round: held in a register across the merges, it spills.
+template <int G, int J>
+__device__ __forceinline__ void merge_misses(const ModelParams& P, BpePage& sh, int64_t base, const int& count, bool back) {
+  const int tid = threadIdx.x, lane = tid & 31, grp = tid / G, gl = tid % G;
+  for (int m0 = 0; m0 < count; m0 += MODEL_THREADS / G) {
+    const int mi = m0 + grp;
+    const bool active0 = mi < count;
+    const int k = active0 ? (back ? sh.list[BpePage::SPAN - 1 - mi] : sh.list[mi]) : 0;
+    const int s = active0 ? sh.pt[k] : 0, e = active0 ? sh.pt[k + 1] : 0;
+    const bool whole = whole_word_gate(P, sh.byte, sh.tok, s, e, active0 && gl == 0 && !is_piece(sh, base, P.n, s, e), lane & ~(G - 1));
+    const bool active = active0 && !whole;
+    coop_bpe<G, J>(P.t, sh.byte, sh.tok, s, e, active, gl);
+    __syncwarp();
+    // long numbers rarely repeat: publishing them only fills the table
+    const bool numeric = active0 && (e - s) >= 5 && (unsigned)(sh.byte[s + 1] - '0') < 10u && (unsigned)(sh.byte[e - 1] - '0') < 10u;
+    if (active0 && gl == 0) wc_publish(P, sh.byte, sh.tok, s, e, numeric || (P.t.ignore_merges && is_piece(sh, base, P.n, s, e)));
+  }
+}
+
+// BPE P3 (word cache, one pre-token per thread), P4a (misses of <= 32 bytes, G lanes each), P4b (33..256 bytes, a warp each)
+__device__ __forceinline__ void resolve_bpe(const ModelParams& P, BpePage& sh, int64_t t, int64_t base) {
+  const int Pproc = page_span<MODEL_BPE>(sh).pproc;
+  constexpr int SPAN = BpePage::SPAN, NWARPS = MODEL_THREADS / 32;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  // (static assignment: a lookup costs the same for every lane, so the warp stays converged)
+  for (int k0 = 0; k0 < Pproc; k0 += MODEL_THREADS) {
+    const int k = k0 + tid;
+    int kind = 0;  // 0 = resolved / nothing to do, 1 = miss (<= 32 bytes), 2 = medium (33..256 bytes)
+    if (k < Pproc) {
+      const int s = sh.pt[k], e = sh.pt[k + 1], len = e - s;
+      if (added_at(P, sh, s)) sh.tok[s] = tok_pack(added_id(P, t, s), len);   // an added token: one token, whatever the model says
+      else if (len > LONG_PRETOK_MIN) kind = 0;  // resolved by the pre-pass
+      else if (len > THREAD_PATH_MAX) kind = 2;
+      else kind = wc_lookup(P, sh.byte, sh.tok, s, len, P.t.ignore_merges && is_piece(sh, base, P.n, s, e)) ? 0 : 1;
+    }
+    // the four groups of a warp step through their merges together, so pre-tokens of similar length should share a
+    // warp: short misses queue from the front of list, longer ones from the back
+    const bool longer = kind == 1 && (int)sh.pt[k + 1] - (int)sh.pt[k] > P4_SPLIT_BYTES;
+    warp_enqueue(sh.list, &sh.nmiss, kind == 1 && !longer, k, false);
+    warp_enqueue(sh.list + SPAN - 1, &sh.nmiss_hi, longer, k, true);
+    warp_enqueue(sh.mq, &sh.nmq, kind == 2, k, false);
+  }
+  __syncthreads();
+  // longer pre-tokens (17..32 bytes: rare, many rounds) by lane groups
+  merge_misses<8, THREAD_PATH_MAX / 8>(P, sh, base, sh.nmiss_hi, true);
+  // short ones (<= 16 bytes: nearly all misses) with fewer positions per lane.  (One THREAD per short miss, 32 words per
+  // warp with the pair ranks in shared memory, needs 4-5x fewer instructions per word but was slower when tried, with the
+  // cache on and off: the page waits for its longest chain of dependent probes, and a lane group's chain is the shortest.)
+  merge_misses<P4_SHORT_G, (P4_SPLIT_BYTES + P4_SHORT_G - 1) / P4_SHORT_G>(P, sh, base, sh.nmiss, false);
+  const int nmq = sh.nmq;
+  for (int qi = warp; qi < nmq; qi += NWARPS) {
+    const int k = sh.mq[qi], s = sh.pt[k], e = sh.pt[k + 1];
+    const bool active = !whole_word_gate(P, sh.byte, sh.tok, s, e, lane == 0 && !is_piece(sh, base, P.n, s, e), 0);
+    coop_bpe<32, LONG_PRETOK_MIN / 32>(P.t, sh.byte, sh.tok, s, e, active, lane);
+  }
+}
+
+// WordPiece P3 (word cache, one split per thread), P4 (misses, one thread per split), and the characters of a split
+// that runs past the halo
+__device__ __forceinline__ void resolve_wordpiece(const ModelParams& P, WpPage& sh, int64_t t, int64_t base) {
+  const PageSpan sp = page_span<MODEL_WORDPIECE>(sh);
+  const int tid = threadIdx.x, lane = tid & 31;
+  for (int k0 = 0; k0 < sp.pproc; k0 += MODEL_THREADS) {
+    const int k = k0 + tid;
+    bool miss = false;
+    if (k < sp.pproc) {
+      const int s = sh.pt[k], e = sh.pt[k + 1], len = e - s;
+      if (added_at(P, sh, s)) sh.tok[s] = tok_pack(added_id(P, t, s), len);
+      else if (bit_at(sh.keptb, s)) miss = !wc_lookup(P, sh.byte, sh.tok, s, len, false);  // not removed whitespace
+    }
+    warp_enqueue(sh.list, &sh.nmiss, miss, k, false);
+  }
+  __syncthreads();
+  const int nmiss = sh.nmiss;
+  while (true) {
+    const int mi = atomicAdd(&sh.next, 1);
+    if (mi >= nmiss) break;
+    const int k = sh.list[mi];
+    const int s = sh.pt[k], e = sh.pt[k + 1], len = e - s;
+    // chars = lead bytes in [s, e)
+    const int chars = bit_rank_incl(sh.lpref, sh.leadb, e - 1) - (s ? bit_rank_incl(sh.lpref, sh.leadb, s - 1) : 0);
+    bool bad = chars > (int)P.t.max_chars;
+    if (!bad) {
+      int start = s;
+      while (start < e) {
+        uint32_t node = (start == s) ? 0u : 1u, best_id = 0;
+        int best_end = -1;
+        for (int p = start; p < e; ++p) {
+          const uint32_t key = (node << 8) | sh.byte[p];
+          uint32_t slot = edge_hash(node, sh.byte[p]) & P.t.edge_mask;
+          uint4 en;
+          while (true) {
+            en = __ldg(P.t.edge_tbl + slot);
+            if (en.x == key || en.x == EMPTY_KEY) break;
+            slot = (slot + 1) & P.t.edge_mask;
           }
-          kind = hit ? 0 : 1;
+          if (en.x == EMPTY_KEY) break;
+          node = en.y;
+          if (en.z != EMPTY_KEY) { best_id = en.z; best_end = p + 1; }
         }
-      }
-      // warp-aggregated queue appends
-      // the four groups of a warp step through their merges together, so pre-tokens of similar length should share a
-      // warp: short misses queue from the front of s_miss, longer ones from the back
-      const bool longer = kind == 1 && (int)s_pt[k + 1] - (int)s_pt[k] > P4_SPLIT_BYTES;
-      const unsigned mm = __ballot_sync(0xFFFFFFFFu, kind == 1 && !longer), mh = __ballot_sync(0xFFFFFFFFu, longer),
-                     mq = __ballot_sync(0xFFFFFFFFu, kind == 2);
-      int bm = 0, bh = 0, bq = 0;
-      if (lane == 0) {
-        if (mm) bm = atomicAdd(&s_nmiss, __popc(mm));
-        if (mh) bh = atomicAdd(&s_nmiss_hi, __popc(mh));
-        if (mq) bq = atomicAdd(&s_nmq, __popc(mq));
-      }
-      bm = __shfl_sync(0xFFFFFFFFu, bm, 0); bh = __shfl_sync(0xFFFFFFFFu, bh, 0); bq = __shfl_sync(0xFFFFFFFFu, bq, 0);
-      if (kind == 1 && !longer) s_miss[bm + __popc(mm & ((1u << lane) - 1u))] = (uint16_t)k;
-      if (longer) s_miss[SPAN - 1 - (bh + __popc(mh & ((1u << lane) - 1u)))] = (uint16_t)k;
-      if (kind == 2) s_mq[bq + __popc(mq & ((1u << lane) - 1u))] = (uint16_t)k;
-    }
-    __syncthreads();
-    // -------------------------------------------------------------- P4a: misses, G lanes per pre-token (<= 32 bytes)
-    {
-      const int n_short = s_nmiss, n_longer = s_nmiss_hi;
-      // G lanes x J positions resolve the logical misses [0, count): longer ones live at the back of s_miss
-      auto run_misses = [&](auto gtag, auto jtag, int count, bool back) {
-        constexpr int G = decltype(gtag)::value, J = decltype(jtag)::value;
-        const int grp = tid / G, gl = tid % G;
-        for (int m0 = 0; m0 < count; m0 += MODEL_THREADS / G) {
-          const int mi = m0 + grp;
-          const bool active0 = mi < count;
-          const int k = active0 ? (back ? s_miss[SPAN - 1 - mi] : s_miss[mi]) : 0;
-          const int s = active0 ? s_pt[k] : 0, e = active0 ? s_pt[k + 1] : 0;
-          bool active = active0;
-          if (P.t.ignore_merges) {  // models/bpe/model.rs:558-567: the whole pre-token is a vocabulary entry -> one token
-            int whole = 0;
-            if (active0 && gl == 0 && !is_piece(s, e)) whole = vocab_whole_word(P.t, s_byte, s, e - s, s_tok) ? 1 : 0;
-            whole = __shfl_sync(0xFFFFFFFFu, whole, lane & ~(G - 1));
-            active = active0 && !whole;
-          }
-          coop_bpe<G, J>(P.t, s_byte, s_tok, s, e, active, gl);
-          __syncwarp();
-          // long numbers rarely repeat: publishing them only fills the table
-          const bool numeric = active0 && (e - s) >= 5 && (unsigned)(s_byte[s + 1] - '0') < 10u && (unsigned)(s_byte[e - 1] - '0') < 10u;
-          if (P.wcache_on && active0 && gl == 0 && e - s <= WC_MAX_BYTES && !numeric && !(P.t.ignore_merges && is_piece(s, e))) {
-            WordKey key;
-            wc_make_key(s_byte, s, e - s, key);
-            wc_publish(P.wcache, P.wcache_mask, key, s, e, s_tok);
-          }
-        }
-      };
-      // longer pre-tokens (17..32 bytes: rare, many rounds) by lane groups
-      run_misses(IntTag<8>{}, IntTag<THREAD_PATH_MAX / 8>{}, n_longer, true);
-      // short ones (<= 16 bytes: nearly all misses) with fewer positions per lane.  (One THREAD per short miss, 32 words per
-      // warp with the pair ranks in shared memory, needs 4-5x fewer instructions per word but was slower when tried, with the
-      // cache on and off: the page waits for its longest chain of dependent probes, and a lane group's chain is the shortest.)
-      run_misses(IntTag<P4_SHORT_G>{}, IntTag<(P4_SPLIT_BYTES + P4_SHORT_G - 1) / P4_SHORT_G>{}, n_short, false);
-    }
-    // -------------------------------------------------------------- P4b: one warp per longer pre-token (33..256 bytes)
-    {
-      const int nmq = s_nmq;
-      for (int qi = warp; qi < nmq; qi += NWARPS) {
-        const int k = s_mq[qi], s = s_pt[k], e = s_pt[k + 1];
-        bool active = true;
-        if (P.t.ignore_merges) {
-          int whole = 0;
-          if (lane == 0 && !is_piece(s, e)) whole = vocab_whole_word(P.t, s_byte, s, e - s, s_tok) ? 1 : 0;
-          whole = __shfl_sync(0xFFFFFFFFu, whole, 0);
-          active = !whole;
-        }
-        coop_bpe<32, LONG_PRETOK_MIN / 32>(P.t, s_byte, s_tok, s, e, active, lane);
+        if (best_end < 0) { bad = true; break; }
+        sh.tok[start] = tok_pack(best_id, best_end - start);
+        start = best_end;
       }
     }
-  } else {
-    // -------------------------------------------------------------- WordPiece P3: word cache, one split per thread
-    for (int k0 = 0; k0 < Pproc; k0 += MODEL_THREADS) {
-      const int k = k0 + tid;
-      bool miss = false;
-      if (k < Pproc) {
-        const int s = s_pt[k], e = s_pt[k + 1], len = e - s;
-        if (added_at(s)) s_tok[s] = tok_pack(added_id(s), len);
-        else if ((s_keptb[s >> 5] >> (s & 31)) & 1u) {  // not removed whitespace
-          bool hit = false;
-          if (P.wcache_on && len <= WC_MAX_BYTES) {
-            WordKey key;
-            wc_make_key(s_byte, s, len, key);
-            hit = wc_lookup(P.wcache, P.wcache_mask, key, s, s_tok);
-          }
-          miss = !hit;
-        }
-      }
-      const unsigned mm = __ballot_sync(0xFFFFFFFFu, miss);
-      int bm = 0;
-      if (lane == 0 && mm) bm = atomicAdd(&s_nmiss, __popc(mm));
-      bm = __shfl_sync(0xFFFFFFFFu, bm, 0);
-      if (miss) s_miss[bm + __popc(mm & ((1u << lane) - 1u))] = (uint16_t)k;
+    if (bad) {
+      for (int p = s; p < e; ++p) sh.tok[p] = 0u;
+      sh.tok[s] = tok_pack(P.t.unk_id, len);
     }
-    __syncthreads();
-    // -------------------------------------------------------------- WordPiece P4: misses, one thread per split
-    const int nmiss = s_nmiss;
-    while (true) {
-      const int mi = atomicAdd(&s_next, 1);
-      if (mi >= nmiss) break;
-      const int k = s_miss[mi];
-      const int s = s_pt[k], e = s_pt[k + 1], len = e - s;
-      // chars = lead bytes in [s, e)
-      int chars = (int)s_lpref[(e - 1) >> 5] + __popc(s_leadb[(e - 1) >> 5] & mask_le((e - 1) & 31)) -
-                  ((int)s_lpref[s >> 5] + __popc(s_leadb[s >> 5] & (mask_le(s & 31) >> 1)));
-      bool bad = chars > (int)P.t.max_chars;
-      if (!bad) {
-        int start = s;
-        while (start < e) {
-          uint32_t node = (start == s) ? 0u : 1u, best_id = 0;
-          int best_end = -1;
-          for (int p = start; p < e; ++p) {
-            const uint32_t key = (node << 8) | s_byte[p];
-            uint32_t slot = edge_hash(node, s_byte[p]) & P.t.edge_mask;
-            uint4 en;
-            while (true) {
-              en = __ldg(P.t.edge_tbl + slot);
-              if (en.x == key || en.x == EMPTY_KEY) break;
-              slot = (slot + 1) & P.t.edge_mask;
-            }
-            if (en.x == EMPTY_KEY) break;
-            node = en.y;
-            if (en.z != EMPTY_KEY) { best_id = en.z; best_end = p + 1; }
-          }
-          if (best_end < 0) { bad = true; break; }
-          s_tok[start] = tok_pack(best_id, best_end - start);
-          start = best_end;
-        }
-      }
-      if (bad) {
-        for (int p = s; p < e; ++p) s_tok[p] = 0u;
-        s_tok[s] = tok_pack(P.t.unk_id, len);
-      }
-      if (P.wcache_on && len <= WC_MAX_BYTES) {
-        WordKey key;
-        wc_make_key(s_byte, s, len, key);
-        wc_publish(P.wcache, P.wcache_mask, key, s, e, s_tok);
-      }
-    }
-    // a LONG split (> 416 bytes) has more than max_input_chars_per_word (<= 100 * 4 bytes) characters: it is [UNK];
-    // count its characters for the end offset
-    if (is_long) {
-      const int64_t ls = base + s_pt[Pn - 1], le = s_long_end;
-      int cnt = 0;
-      for (int64_t p = ls + tid; p < le; p += MODEL_THREADS) cnt += ((__ldg(P.bytes + p) & 0xC0u) != 0x80u);
+    wc_publish(P, sh.byte, sh.tok, s, e, false);
+  }
+  // a LONG split (> 416 bytes) has more than max_input_chars_per_word (<= 100 * 4 bytes) characters: it is [UNK];
+  // count its characters for the end offset
+  if (sp.is_long) {
+    const int64_t ls = base + sh.pt[sh.npt - 1], le = sh.long_end;
+    int cnt = 0;
+    for (int64_t p = ls + tid; p < le; p += MODEL_THREADS) cnt += ((__ldg(P.bytes + p) & 0xC0u) != 0x80u);
 #pragma unroll
-      for (int sft = 16; sft >= 1; sft >>= 1) cnt += __shfl_xor_sync(0xFFFFFFFFu, cnt, sft);
-      if (lane == 0) atomicAdd(&s_long_chars, cnt);
-    }
+    for (int sft = 16; sft >= 1; sft >>= 1) cnt += __shfl_xor_sync(0xFFFFFFFFu, cnt, sft);
+    if (lane == 0) atomicAdd(&sh.long_chars, cnt);
   }
-  __syncthreads();
+}
 
-  // ---------------------------------------------------------------- P5: token bitmap and count
-  for (int row = warp; row < NW; row += NWARPS) {
-    int pos = row * 32 + lane;
-    bool tok = pos >= first && pos < Eproc && tok_len(s_tok[pos]) != 0;
-    uint32_t tb = __ballot_sync(0xFFFFFFFFu, tok);
-    if (lane == 0) s_tokb[row] = tb;
+// P5/P6: token bitmap, its prefix, the list of token positions and the page's token count (no ordering between pages:
+// an in-order look-back chain stalls every page behind the slowest of the pages in flight)
+template <int MODEL, class S>
+__device__ __forceinline__ void count_tokens(const ModelParams& P, S& sh, int64_t t, int64_t base) {
+  const int tid = threadIdx.x, lane = tid & 31;
+  const PageSpan sp = page_span<MODEL>(sh);
+  for (int row = tid >> 5; row < S::NW; row += MODEL_THREADS / 32) {
+    const int pos = row * 32 + lane;
+    const uint32_t tb = __ballot_sync(0xFFFFFFFFu, pos >= sp.first && pos < sp.eproc && tok_len(sh.tok[pos]) != 0);
+    if (lane == 0) sh.tokb[row] = tb;
   }
   __syncthreads();
-  const bool long_kept = MODEL == MODEL_WORDPIECE && is_long && ((s_keptb[s_pt[Pn - 1] >> 5] >> (s_pt[Pn - 1] & 31)) & 1u);
-  if (warp == 0) {
-    int tot = warp_prefix_words(s_tokb, s_tpref, NW, lane);
-    if (lane == 0) s_ntok = tot;
+  if (tid < 32) {
+    const int tot = warp_prefix_words(sh.tokb, sh.tpref, S::NW, lane);
+    if (lane == 0) sh.ntok = tot;
   }
   __syncthreads();
-  {
-    // compact list of token positions
-    for (int row = warp; row < NW; row += NWARPS) {
-      const uint32_t tb = s_tokb[row];
-      if ((tb >> lane) & 1u) s_tokpos[s_tpref[row] + __popc(tb & ((1u << lane) - 1u))] = (uint16_t)(row * 32 + lane);
-    }
-    // ---------------------------------------------------------------- P6: page token count (no ordering between pages:
-    // an in-order look-back chain stalls every page behind the slowest of the pages in flight)
-    if (tid == 0) {
-      const int A = s_ntok + ((MODEL == MODEL_WORDPIECE && long_kept) ? 1 : 0) + (MODEL == MODEL_BPE ? s_lcum[n_longs] : 0);
-      s_ntot = A;
-      s_excl = (unsigned long long)(base + first);  // provisional slot of the page's first token
-      P.tile_count[t] = (uint32_t)A;
-      P.tile_first[t] = (uint32_t)(base + first);
-    }
+  for (int row = tid >> 5; row < S::NW; row += MODEL_THREADS / 32) {
+    const uint32_t tb = sh.tokb[row];
+    if ((tb >> lane) & 1u) sh.list[sh.tpref[row] + __popc(tb & ((1u << lane) - 1u))] = (uint16_t)(row * 32 + lane);
   }
-  __syncthreads();
-  const unsigned long long excl = s_excl;
-  // chars / kept splits of the document that spans into this page, counted from its start (pretok_kernels.cuh K1b)
-  const uint64_t carry = __ldg(P.page_carry + t);
-  int carry_chars = (int)((uint32_t)carry & 0x7FFFFFFFu), carry_starts = (int)(uint32_t)(carry >> 32);
-  if (!((carry >> 31) & 1ull)) {  // no document start earlier in this scan block: add the block's carry
-    const uint64_t bc = __ldg(P.block_carry + (t >> 10));
-    carry_chars += (int)(uint32_t)bc; carry_starts += (int)(uint32_t)(bc >> 32);
+  if (tid == 0) {
+    P.tile_count[t] = (uint32_t)(sh.ntok + long_tokens_before(sh, TILE) + (sp.long_kept ? 1 : 0));
+    P.tile_first[t] = (uint32_t)(base + sp.first);
   }
-  const bool want_off = P.flags & F_OFFSETS, want_wid = P.flags & F_WORD_IDS, byte_off = P.flags & F_BYTE_OFFSETS;
+}
 
-  // ---------------------------------------------------------------- P7: emit tokens in order
-  auto lc_incl = [&](int x) -> int { return (int)s_lpref[x >> 5] + __popc(s_leadb[x >> 5] & mask_le(x & 31)); };
-  auto kept_incl = [&](int x) -> int { return (int)s_spref[x >> 5] + __popc(s_keptb[x >> 5] & mask_le(x & 31)); };
-  auto doc_base = [&](int x) -> int {  // last doc start at or before x inside the page, or -1
-    int xx = x < TILE ? x : TILE - 1;
-    uint32_t m = s_dsb[xx >> 5] & mask_le(xx & 31);
-    return m ? (xx & ~31) + 31 - __clz((int)m) : (int)s_dlast[xx >> 5];
-  };
-  auto emit = [&](unsigned long long out, uint32_t id, int ts, int64_t tend_abs, int end_chars_in_page, bool end_known) {
-    // ts: token start (page-relative); tend_abs: absolute end byte; end_chars_in_page: lc_incl(e-1) if end_known
-    P.ids[out] = (P.flag_added && ts < TILE && added_at(ts)) ? (id | 0x80000000u) : id;
-    const int D = doc_base(ts);
-    if (want_off) {
-      uint32_t o0, o1;
-      if (!byte_off) {
-        const int cb = D >= 0 ? lc_incl(D) - 1 : -carry_chars;  // chars before the doc start, page-relative
-        o0 = (uint32_t)(lc_incl(ts) - 1 - cb);
-        o1 = (uint32_t)(end_chars_in_page - cb);
-      } else {
-        int64_t ds = D >= 0 ? base + D : s_span_doc_start;
-        int64_t gs = base + ts, ge = tend_abs;
-        while (gs > 0 && (__ldg(P.bytes + gs) & 0xC0u) == 0x80u) --gs;
-        while (ge < n && (__ldg(P.bytes + ge) & 0xC0u) == 0x80u) ++ge;
-        o0 = (uint32_t)(gs - ds); o1 = (uint32_t)(ge - ds);
-      }
-      (void)end_known;
-      if (P.prefix_bits) {  // offsets were computed on the document WITH its inserted space: map back (normalizer.rs:503-514)
-        const int64_t dsa = D >= 0 ? base + D : s_span_doc_start;
-        if ((__ldg(P.prefix_bits + (dsa >> 5)) >> (dsa & 31)) & 1u) {
-          if (o1 == 1u && byte_off) {  // the token is the inserted space alone: it is aligned to the whole first character
-            int64_t ge2 = dsa + 2;
-            while (ge2 < n && (__ldg(P.bytes + ge2) & 0xC0u) == 0x80u) ++ge2;
-            o1 = (uint32_t)(ge2 - dsa);
-          }
-          o0 = o0 ? o0 - 1u : 0u;
-          o1 = o1 > 2u ? o1 - 1u : 1u;
-          if (byte_off && o1 < 1u) o1 = 1u;
-        }
-      }
-      reinterpret_cast<uint2*>(P.offsets)[out] = make_uint2(o0, o1);
-    }
-    if (want_wid) {
-      // kept splits before the doc start (the split AT the doc start may itself be removed whitespace)
-      const int wb = D >= 0 ? kept_incl(D) - (int)((s_keptb[D >> 5] >> (D & 31)) & 1u) : -carry_starts;
-      P.word_ids[out] = (uint32_t)(kept_incl(ts) - 1 - wb);
-    }
-  };
-  const int n_normal = s_ntok;
-  for (int j = tid; j < n_normal; j += MODEL_THREADS) {
-    const int pos = s_tokpos[j];
-    const unsigned long long out = excl + (unsigned long long)(j + long_tokens_before(pos));
-    const uint32_t tk = s_tok[pos];
+// P7: ids, offsets and word ids of the page's tokens at the provisional slots from base + first on
+template <int MODEL, class S>
+__device__ __forceinline__ void emit_tokens(const ModelParams& P, const S& sh, int64_t base) {
+  const PageSpan sp = page_span<MODEL>(sh);
+  const unsigned long long excl = (unsigned long long)(base + sp.first);
+  const int n_normal = sh.ntok;
+  for (int j = threadIdx.x; j < n_normal; j += MODEL_THREADS) {
+    const int pos = sh.list[j];
+    const uint32_t tk = sh.tok[pos];
     const int e = pos + tok_len(tk);
-    emit(out, tok_id(tk), pos, base + e, lc_incl(e - 1), true);
+    emit_token(P, sh, base, excl + (unsigned long long)(j + long_tokens_before(sh, pos)), tok_id(tk), pos,
+               bit_rank_incl(sh.lpref, sh.leadb, e - 1), base + e);
   }
-  if (MODEL == MODEL_BPE) {
-    // tokens of the long pre-tokens, produced by the pre-pass (relative to the pre-token start)
-    for (int a = 0; a < n_longs; ++a) {
-      const int ls = s_pt[s_lk[a]];
-      const int ntl = s_lcum[a + 1] - s_lcum[a];
+  if constexpr (MODEL == MODEL_BPE) {
+    // tokens of the long pre-tokens, produced by the pre-pass (positions relative to the pre-token start)
+    for (int a = 0; a < sh.nl; ++a) {
+      const int ls = sh.pt[sh.lk[a]];
+      const int ntl = sh.lcum[a + 1] - sh.lcum[a];
       if (ntl == 0) continue;
-      const uint4* __restrict__ lo = P.long_out + s_loff[a];
-      const int nb = ls == 0 ? 0 : (int)s_tpref[(ls - 1) >> 5] + __popc(s_tokb[(ls - 1) >> 5] & mask_le((ls - 1) & 31));
-      const unsigned long long obase = excl + (unsigned long long)(nb + s_lcum[a]);
-      const int D = doc_base(ls);
-      const int cb = D >= 0 ? lc_incl(D) - 1 : -carry_chars;
-      const int X = lc_incl(ls) - 1 - cb;  // char index of the pre-token's first char inside its document
-      const int wb = D >= 0 ? kept_incl(D) - (int)((s_keptb[D >> 5] >> (D & 31)) & 1u) : -carry_starts;
-      const uint32_t wid = (uint32_t)(kept_incl(ls) - 1 - wb);
-      const int64_t ds = D >= 0 ? base + D : s_span_doc_start;
-      for (int k = tid; k < ntl; k += MODEL_THREADS) {
+      const uint4* __restrict__ lo = P.long_out + sh.loff[a];
+      const int nb = ls == 0 ? 0 : bit_rank_incl(sh.tpref, sh.tokb, ls - 1);
+      const unsigned long long obase = excl + (unsigned long long)(nb + sh.lcum[a]);
+      const int X = bit_rank_incl(sh.lpref, sh.leadb, ls) - 1;  // chars of the page before the pre-token
+      const DocOrigin o = doc_origin(P, sh, base, ls);
+      for (int k = threadIdx.x; k < ntl; k += MODEL_THREADS) {
         const uint4 r = lo[k];
         P.ids[obase + k] = r.x;
-        if (want_off) {
-          uint32_t o0, o1;
-          if (!byte_off) { o0 = (uint32_t)X + r.z; o1 = (uint32_t)X + r.w; }
-          else {
-            int64_t gs = base + ls + (k ? (int64_t)lo[k - 1].y : 0), ge = base + ls + (int64_t)r.y;
-            while (gs > 0 && (__ldg(P.bytes + gs) & 0xC0u) == 0x80u) --gs;
-            while (ge < n && (__ldg(P.bytes + ge) & 0xC0u) == 0x80u) ++ge;
-            o0 = (uint32_t)(gs - ds); o1 = (uint32_t)(ge - ds);
-          }
-          if (P.prefix_bits && ((__ldg(P.prefix_bits + (ds >> 5)) >> (ds & 31)) & 1u)) {
-            if (o1 == 1u && byte_off) {
-              int64_t ge2 = ds + 2;
-              while (ge2 < n && (__ldg(P.bytes + ge2) & 0xC0u) == 0x80u) ++ge2;
-              o1 = (uint32_t)(ge2 - ds);
-            }
-            o0 = o0 ? o0 - 1u : 0u;
-            o1 = o1 > 2u ? o1 - 1u : 1u;
-          }
-          reinterpret_cast<uint2*>(P.offsets)[obase + k] = make_uint2(o0, o1);
-        }
-        if (want_wid) P.word_ids[obase + k] = wid;
+        place_token(P, o, obase + k, X + (int)r.z, X + (int)r.w, base + ls + (k ? (int64_t)lo[k - 1].y : 0), base + ls + (int64_t)r.y);
       }
     }
-  }
-  if (MODEL == MODEL_WORDPIECE && long_kept && tid == 0) {
-    const int ls = s_pt[Pn - 1];
-    const unsigned long long out = excl + (unsigned long long)(s_ntot - 1);
+  } else if (sp.long_kept && threadIdx.x == 0) {
     // chars up to the end of the long split = chars before it in the page + its own
-    const int end_chars = lc_incl(ls) - 1 + s_long_chars;
-    emit(out, P.t.unk_id, ls, s_long_end, end_chars, true);
+    const int ls = sh.pt[sh.npt - 1];
+    emit_token(P, sh, base, excl + (unsigned long long)sh.ntok, P.t.unk_id, ls,
+               bit_rank_incl(sh.lpref, sh.leadb, ls) - 1 + sh.long_chars, sh.long_end);
   }
+}
 
-  // ---------------------------------------------------------------- P8: row_ptr of the documents starting in this page
-  {
-    const uint32_t fd = __ldg(P.page_first_doc + t);
-    for (uint64_t d = (uint64_t)fd + tid; d <= P.n_docs; d += MODEL_THREADS) {
-      const int64_t pos = (int64_t)__ldg(P.doc_off + d) - base;
-      if (pos >= TILE) break;
-      // tokens that start before `pos` (a doc start is a pre-token start, so no token straddles it)
-      const int before = pos == 0 ? 0 : (int)s_tpref[(pos - 1) >> 5] + __popc(s_tokb[(pos - 1) >> 5] & mask_le((int)((pos - 1) & 31)));
-      P.row_ptr[d] = (unsigned long long)(before + long_tokens_before((int)pos));  // page-local; row_ptr_fix_kernel adds the page's base
-    }
+// P8: row_ptr of the documents starting in this page, page-local (row_ptr_fix_kernel adds the page's base)
+template <class S>
+__device__ __forceinline__ void write_row_ptr(const ModelParams& P, const S& sh, int64_t t, int64_t base) {
+  const uint32_t fd = __ldg(P.page_first_doc + t);
+  for (uint64_t d = (uint64_t)fd + threadIdx.x; d <= P.n_docs; d += MODEL_THREADS) {
+    const int64_t pos = (int64_t)__ldg(P.doc_off + d) - base;
+    if (pos >= TILE) break;
+    // tokens that start before `pos` (a doc start is a pre-token start, so no token straddles it)
+    const int before = pos == 0 ? 0 : bit_rank_incl(sh.tpref, sh.tokb, (int)pos - 1);
+    P.row_ptr[d] = (unsigned long long)(before + long_tokens_before(sh, (int)pos));
   }
+}
+
+constexpr int MODEL_MINBLOCKS = 8;  // 8 blocks/SM (32 regs, small spills) rather than 5 (48 regs): the kernel is latency-bound
+template <int MODEL>
+__global__ void __launch_bounds__(MODEL_THREADS, MODEL_MINBLOCKS) model_tile_kernel(const ModelParams P) {
+  __shared__ __align__(16) PageState<MODEL> sh;
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    sh.tile = (int)blockIdx.x;
+    sh.nmiss = 0;
+    if constexpr (MODEL == MODEL_BPE) { sh.nmiss_hi = 0; sh.nmq = 0; sh.anysoft = 0; sh.nl = 0; sh.lcum[0] = 0; }
+    else { sh.next = 0; sh.long_chars = 0; }
+  }
+  __syncthreads();
+  const int64_t t = sh.tile;
+  if (t >= P.n_tiles) return;
+  const int64_t base = t * TILE;
+
+  stage_page<MODEL>(P, sh, t, base);
+  __syncthreads();
+  if constexpr (MODEL == MODEL_BPE) {
+    collect_long_pretokens(P, sh, t, base);
+    resolve_bpe(P, sh, t, base);
+  } else {
+    resolve_wordpiece(P, sh, t, base);
+  }
+  __syncthreads();
+  count_tokens<MODEL>(P, sh, t, base);
+  __syncthreads();
+  emit_tokens<MODEL>(P, sh, base);
+  write_row_ptr(P, sh, t, base);
 }
 
 
@@ -892,26 +899,30 @@ __global__ void __launch_bounds__(MODEL_THREADS, MODEL_MINBLOCKS) model_tile_ker
 // Exclusive scan of the page token counts (two levels of 1024), then compaction of the provisional slots.
 constexpr int TSCAN = 1024;
 
+// exclusive scan of v over a block of TSCAN threads; s_w: 32 words of shared memory
+__device__ __forceinline__ unsigned long long block_excl_scan(unsigned long long v, unsigned long long* s_w) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  auto warp_incl_scan = [lane](unsigned long long x) {
+#pragma unroll
+    for (int s = 1; s < 32; s <<= 1) { unsigned long long o = __shfl_up_sync(0xFFFFFFFFu, x, s); if (lane >= s) x += o; }
+    return x;
+  };
+  const unsigned long long inc = warp_incl_scan(v);
+  if (lane == 31) s_w[warp] = inc;
+  __syncthreads();
+  if (warp == 0) { const unsigned long long w = s_w[lane]; s_w[lane] = warp_incl_scan(w) - w; }
+  __syncthreads();
+  return s_w[warp] + inc - v;
+}
+
 __global__ void __launch_bounds__(TSCAN) tile_scan_block_kernel(const uint32_t* __restrict__ cnt, unsigned long long* __restrict__ local_excl,
                                                                 unsigned long long* __restrict__ block_sum, int64_t n_tiles) {
   __shared__ unsigned long long s_w[32];
   const int64_t i = (int64_t)blockIdx.x * TSCAN + threadIdx.x;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const unsigned long long v = i < n_tiles ? (unsigned long long)cnt[i] : 0ull;
-  unsigned long long inc = v;
-#pragma unroll
-  for (int s = 1; s < 32; s <<= 1) { unsigned long long o = __shfl_up_sync(0xFFFFFFFFu, inc, s); if (lane >= s) inc += o; }
-  if (lane == 31) s_w[warp] = inc;
-  __syncthreads();
-  if (warp == 0) {
-    unsigned long long w = s_w[lane], wi = w;
-#pragma unroll
-    for (int s = 1; s < 32; s <<= 1) { unsigned long long o = __shfl_up_sync(0xFFFFFFFFu, wi, s); if (lane >= s) wi += o; }
-    s_w[lane] = wi - w;
-    if (lane == 31) block_sum[blockIdx.x] = wi;
-  }
-  __syncthreads();
-  if (i < n_tiles) local_excl[i] = s_w[warp] + inc - v;
+  const unsigned long long ex = block_excl_scan(v, s_w);
+  if (i < n_tiles) local_excl[i] = ex;
+  if (threadIdx.x == TSCAN - 1) block_sum[blockIdx.x] = ex + v;
 }
 
 __global__ void __launch_bounds__(TSCAN) tile_scan_top_kernel(unsigned long long* __restrict__ block_sum, int64_t n_blocks, unsigned long long* __restrict__ total) {
@@ -919,26 +930,14 @@ __global__ void __launch_bounds__(TSCAN) tile_scan_top_kernel(unsigned long long
   __shared__ unsigned long long s_run;
   if (threadIdx.x == 0) s_run = 0;
   __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int64_t b0 = 0; b0 < n_blocks; b0 += TSCAN) {
     const int64_t i = b0 + threadIdx.x;
     const unsigned long long v = i < n_blocks ? block_sum[i] : 0ull;
-    unsigned long long inc = v;
-#pragma unroll
-    for (int s = 1; s < 32; s <<= 1) { unsigned long long o = __shfl_up_sync(0xFFFFFFFFu, inc, s); if (lane >= s) inc += o; }
-    if (lane == 31) s_w[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-      unsigned long long w = s_w[lane], wi = w;
-#pragma unroll
-      for (int s = 1; s < 32; s <<= 1) { unsigned long long o = __shfl_up_sync(0xFFFFFFFFu, wi, s); if (lane >= s) wi += o; }
-      s_w[lane] = wi - w;
-    }
-    __syncthreads();
+    const unsigned long long ex = block_excl_scan(v, s_w);
     const unsigned long long run = s_run;
-    if (i < n_blocks) block_sum[i] = run + s_w[warp] + inc - v;  // exclusive, in place
+    if (i < n_blocks) block_sum[i] = run + ex;  // exclusive, in place
     __syncthreads();
-    if (threadIdx.x == TSCAN - 1) s_run = run + s_w[warp] + inc;
+    if (threadIdx.x == TSCAN - 1) s_run = run + ex + v;
     __syncthreads();
   }
   if (threadIdx.x == 0) *total = s_run;
