@@ -8,10 +8,12 @@ Python lists, one input at a time:
     Encoding::truncate / merge_with         tokenizer/encoding.rs:307-388, 408-463
     PostProcessor::process                  tokenizer/mod.rs:126-148     sequence ids, type ids, merge of the pieces
     templates as piece lists                processors/template.rs:544-643, bert.rs:51-, roberta.rs:66-
-    ByteLevel::process_offsets              pre_tokenizers/byte_level.rs:202-234
+The rules both paths share (truncation spans, the special-token count, offset trimming) live in tokenizer.py.
 All tokenization still happens in the engine: this module only rearranges its output.
 """
 import copy
+import numpy as np
+from .tokenizer import trim_spans, truncation_budget, truncation_spans
 
 
 class PE:
@@ -45,34 +47,11 @@ def special_piece(token_id, type_id):
 
 def truncate(pe, max_len, stride, direction):
     """Encoding::truncate (encoding.rs:307-388), in place"""
-    n = len(pe)
-    if max_len >= n:
+    if max_len >= len(pe):
         return
-    if max_len == 0:
-        whole = pe.slice(0, n)
-        whole.overflowing = pe.overflowing
-        empty = PE(ld=None if pe.ld is None else [], tr=None if pe.tr is None else [])
-        for f in PE.__slots__:
-            setattr(pe, f, getattr(empty, f))
-        pe.overflowing = [whole]
-        return
-    if stride >= max_len:
-        raise ValueError(f"`stride` must be strictly less than `max_len={max_len}` (the maximum length minus the special tokens)")
-    step, parts = max_len - stride, []
-    if direction == "right":
-        for a in range(0, n, step):
-            b = min(a + max_len, n)
-            parts.append((a, b))
-            if b == n:
-                break
-    else:
-        for stop in range(n, 0, -step):
-            a = max(stop - max_len, 0)
-            parts.append((a, stop))
-            if a == 0:
-                break
-    new = pe.slice(*parts[0])
-    new.overflowing = [pe.slice(a, b) for a, b in parts[1:]]
+    spans = truncation_spans(len(pe), max_len, stride, direction)
+    new = pe.slice(*spans[0])
+    new.overflowing = [pe.slice(a, b) for a, b in spans[1:]]
     for f in PE.__slots__:
         setattr(pe, f, getattr(new, f))
 
@@ -133,21 +112,13 @@ def merge_with(acc, pair):
 
 
 def trim(pe, add_prefix_space):
-    """process_offsets (byte_level.rs:202-234) on one encoding and its overflowing parts"""
+    """trim_spans on one encoding and its overflowing parts; the encoding's first token is the first of its sequence"""
     for o in pe.overflowing:
         trim(o, add_prefix_space)
-    if pe.ld is None:
+    if pe.ld is None or not pe.ids:
         return
-    for i, (off, ld, tr) in enumerate(zip(pe.offsets, pe.ld, pe.tr)):
-        o0, o1 = off
-        if ld > 0 or tr > 0:
-            if ld > 0:
-                if (i == 0 or o0 == 0) and add_prefix_space and ld == 1:
-                    ld = 0
-                o0 = min(o0 + ld, o1)
-            if tr > 0 and o1 >= tr:
-                o1 = max(o1 - tr, o0)
-            pe.offsets[i] = (o0, o1)
+    first = np.arange(len(pe)) == 0
+    pe.offsets = [tuple(o) for o in trim_spans(pe.offsets, pe.ld, pe.tr, first, add_prefix_space).tolist()]
 
 
 def post_process(a, b, template, truncation, add_special_tokens):
@@ -159,11 +130,7 @@ def post_process(a, b, template, truncation, add_special_tokens):
         if is_pair and pieces is None:
             raise ValueError("the post-processor has no template for pairs of sequences")
     if truncation is not None:
-        n_added = sum(1 for p in pieces if p[0] == "special") if (pieces is not None and add_special_tokens) else 0
-        tr = dict(truncation, max_length=truncation["max_length"] - n_added) if n_added else truncation
-        if tr["max_length"] < 0:
-            raise ValueError("truncation max_length is smaller than the number of special tokens the post-processor adds")
-        truncate_pair(a, b, tr)
+        truncate_pair(a, b, dict(truncation, max_length=truncation_budget(truncation, template, is_pair, add_special_tokens)))
     seqs = [a] + ([b] if is_pair else [])
     for i, e in enumerate(seqs):  # PostProcessor::process (mod.rs:137-144) / default_process: sequence ids, type ids
         for x in [e] + e.overflowing:

@@ -9,7 +9,7 @@ mirrored here: added-token extraction before it (`added.py`) and the special-tok
 """
 import ctypes, json
 import numpy as np
-from . import _lib, added, pairs
+from . import _lib, added
 from ._lib import B2TError
 
 LLAMA3_PATTERN = (r"(?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\r\n\p{L}\p{N}]?\p{L}+|\p{N}{1,3}| ?[^\s\p{L}\p{N}]+[\r\n]*"
@@ -20,12 +20,14 @@ class UnsupportedConfig(ValueError):
     """The tokenizer.json asks for something outside the accelerated path (the reference handles it on CPU)."""
 
 
-def _pack(strings):
+def _pack(strings, off_dtype):
+    """list of str -> (their UTF-8 bytes back to back as uint8 (a read-only view of one bytes object), off_dtype[n + 1]
+    offsets).  Raises AttributeError for an element that is not a str."""
     bs = [s.encode("utf-8") for s in strings]
-    off = np.zeros(len(bs) + 1, dtype=np.uint32)
+    off = np.zeros(len(bs) + 1, dtype=off_dtype)
     if bs:
         np.cumsum(np.fromiter(map(len, bs), dtype=np.int64, count=len(bs)), out=off[1:])
-    return np.frombuffer(b"".join(bs) + b"\0", dtype=np.uint8).copy(), off
+    return np.frombuffer(b"".join(bs), dtype=np.uint8), off
 
 
 def parse_post_processor(pp):
@@ -185,10 +187,11 @@ NO_WORD = 0xFFFFFFFF  # word id of a token the post-processor added (the referen
 
 
 class _ResultOwner:
-    """Keeps a b2t_result (and the pinned buffers the zero-copy views point into) alive; frees it with the last view holder."""
+    """Keeps a b2t_result (and the pinned buffers the zero-copy views point into) alive; frees it with the last view holder.
+    It also keeps the Tokenizer whose engine made the result, since a result must be freed before its engine."""
 
-    def __init__(self, res):
-        self._res = res
+    def __init__(self, res, tok):
+        self._res, self._tok = res, tok
 
     def __del__(self):
         r, self._res = self._res, None
@@ -197,6 +200,12 @@ class _ResultOwner:
                 _lib.lib().b2t_result_free(r)
             except Exception:
                 pass
+
+
+class _Rows(tuple):
+    """(ids, offsets or None, word ids or None, row_ptr) of one engine call.  `owner`: the _ResultOwner that keeps the
+    arrays valid when they are zero-copy views, else None."""
+    owner = None
 
 
 class BatchEncoding:
@@ -209,6 +218,7 @@ class BatchEncoding:
         self.type_ids, self.special_tokens_mask, self.attention_mask = type_ids, special_tokens_mask, attention_mask
         self.sequence_ids = sequence_ids  # int8, -1 = none (special / pad token); only set for pairs of sequences
         self.token_text = None            # {token index: str}: added tokens whose text is a wider span than their content (lstrip / rstrip)
+        self._owner = None                # the _ResultOwner of the engine result that zero-copy arrays are views of
 
     def _remap_text(self, src, new_to_old):
         """carry src.token_text over to this CSR, whose token i is src's token new_to_old[i]"""
@@ -334,63 +344,81 @@ class Encoding:
         return f"Encoding(num_tokens={len(self)}, attributes=[ids, type_ids, tokens, offsets, attention_mask, special_tokens_mask, overflowing])"
 
 
-def trim_offsets(be, ld, tr, add_prefix_space):
-    """ByteLevel::process_offsets (pre_tokenizers/byte_level.rs:202-234) on the whole CSR: offsets shrink by the token's
-    leading / trailing spaces.  ld / tr: per token, the number of leading / trailing space characters of its text."""
-    if be.offsets is None or be.ids.size == 0:
-        return be
-    ld, tr = ld.astype(np.int64), tr.astype(np.int64)
-    o0, o1 = be.offsets[:, 0].astype(np.int64), be.offsets[:, 1].astype(np.int64)
-    first = np.zeros(be.ids.size, dtype=bool)
-    first[be.row_ptr[:-1][np.diff(be.row_ptr) > 0].astype(np.int64)] = True
-    first |= o0 == 0
-    keep = first & bool(add_prefix_space) & (ld == 1)
+def special_token_count(template, is_pair):
+    """PostProcessor::added_tokens (template.rs:647-653, bert.rs, roberta.rs): the special tokens the template adds to a
+    single sequence or a pair (0 without a template, or for a pair without a pair template)"""
+    pieces = None if template is None else template["pair" if is_pair else "single"]
+    return sum(1 for p in pieces or () if p[0] == "special")
+
+
+def truncation_budget(truncation, template, is_pair, add_special_tokens):
+    """TokenizerImpl::post_process step 1 (tokenizer/mod.rs:1265-1317): truncation's max_length less the special tokens
+    the post-processor will add"""
+    n_added = special_token_count(template, is_pair) if add_special_tokens else 0
+    if truncation["max_length"] < n_added:
+        raise ValueError("truncation max_length is smaller than the number of special tokens the post-processor adds")
+    return truncation["max_length"] - n_added
+
+
+def truncation_spans(n, max_len, stride, direction):
+    """Encoding::truncate (tokenizer/encoding.rs:307-388) on a sequence of n tokens -> [(a, b)]: the kept part first, then
+    the overflowing parts (each max_len long, consecutive ones sharing `stride` tokens)"""
+    if n <= max_len:
+        return [(0, n)]
+    if max_len == 0:
+        return [(0, 0), (0, n)]  # an empty kept part, the whole sequence overflows (encoding.rs:313-317)
+    if stride >= max_len:
+        raise ValueError(f"`stride` must be strictly less than `max_len={max_len}` (the maximum length minus the special tokens)")
+    step, spans = max_len - stride, []
+    if direction == "right":
+        for a in range(0, n, step):
+            b = min(a + max_len, n)
+            spans.append((a, b))
+            if b == n:
+                break
+    else:
+        for stop in range(n, 0, -step):
+            a = max(stop - max_len, 0)
+            spans.append((a, stop))
+            if a == 0:
+                break
+    return spans
+
+
+def trim_spans(offsets, ld, tr, first, add_prefix_space):
+    """ByteLevel::process_offsets (pre_tokenizers/byte_level.rs:202-234): offsets [T, 2] shrink by the token's leading /
+    trailing space characters ld / tr, except that with add_prefix_space a first token of a sequence (`first`), or one
+    at offset 0, keeps a single leading space.  -> uint32 [T, 2]"""
+    ld, tr = np.asarray(ld, dtype=np.int64), np.asarray(tr, dtype=np.int64)
+    o = np.asarray(offsets, dtype=np.int64).reshape(-1, 2)
+    o0, o1 = o[:, 0], o[:, 1]
+    keep = (first | (o0 == 0)) & bool(add_prefix_space) & (ld == 1)
     n0 = np.where((ld > 0) & ~keep, np.minimum(o0 + ld, o1), o0)
     n1 = np.where((tr > 0) & (o1 >= tr), np.maximum(o1 - tr, n0), o1)
-    offs = np.stack([n0, n1], axis=1).astype(np.uint32)
-    out = BatchEncoding(be.ids, offs, be.word_ids, be.row_ptr, be.type_ids, be.special_tokens_mask)
+    return np.stack([n0, n1], axis=1).astype(np.uint32)
+
+
+def trim_offsets(be, ld, tr, add_prefix_space):
+    """trim_spans on the whole CSR.  ld / tr: per token, the number of leading / trailing space characters of its text."""
+    if be.offsets is None or be.ids.size == 0:
+        return be
+    first = np.zeros(be.ids.size, dtype=bool)
+    first[be.row_ptr[:-1][np.diff(be.row_ptr) > 0].astype(np.int64)] = True
+    out = BatchEncoding(be.ids, trim_spans(be.offsets, ld, tr, first, add_prefix_space), be.word_ids, be.row_ptr, be.type_ids,
+                        be.special_tokens_mask)
     out.token_text = be.token_text
     return out
 
 
 def truncate_csr(be, extra, max_length, stride, direction):
-    """Encoding::truncate (tokenizer/encoding.rs:307-388) for every sequence of the CSR: a sequence longer than max_length
-    becomes several rows -- the kept part first, then its overflowing parts (each max_length long, consecutive ones
-    sharing `stride` tokens).  extra: per-token arrays cut the same way.
+    """truncation_spans for every sequence of the CSR: a sequence longer than max_length becomes several rows, the kept
+    part first, then its overflowing parts.  extra: per-token arrays cut the same way.
     -> (BatchEncoding of all parts, extra arrays, part_doc int64[parts] = document of each part)"""
-    counts = np.diff(be.row_ptr).astype(np.int64)
-    starts = be.row_ptr[:-1].astype(np.int64)
     seg_a, seg_b, seg_doc = [], [], []
-    long_docs = np.flatnonzero(counts > max_length)
-    is_long = np.zeros(len(counts), dtype=bool); is_long[long_docs] = True
-    if max_length > 0 and stride >= max_length and long_docs.size:
-        raise ValueError(f"`stride` must be strictly less than `max_len={max_length}` (the maximum length minus the special tokens)")
-    per_doc = {}
-    for d in long_docs.tolist():
-        n = int(counts[d])
-        if max_length == 0:
-            per_doc[d] = [(0, 0), (0, n)]  # an empty kept part, the whole sequence overflows (encoding.rs:313-317)
-            continue
-        step, parts = max_length - stride, []
-        if direction == "right":
-            for a in range(0, n, step):
-                b = min(a + max_length, n)
-                parts.append((a, b))
-                if b == n:
-                    break
-        else:
-            for stop in range(n, 0, -step):
-                a = max(stop - max_length, 0)
-                parts.append((a, stop))
-                if a == 0:
-                    break
-        per_doc[d] = parts
-    for d in range(len(counts)):
-        if not is_long[d]:
-            seg_a.append(int(starts[d])); seg_b.append(int(starts[d] + counts[d])); seg_doc.append(d)
-        else:
-            for a, b in per_doc[d]:
-                seg_a.append(int(starts[d]) + a); seg_b.append(int(starts[d]) + b); seg_doc.append(d)
+    rows = be.row_ptr.astype(np.int64).tolist()
+    for d, (s, e) in enumerate(zip(rows[:-1], rows[1:])):
+        for a, b in truncation_spans(e - s, max_length, stride, direction):
+            seg_a.append(s + a); seg_b.append(s + b); seg_doc.append(d)
     seg_a, seg_b = np.asarray(seg_a, dtype=np.int64), np.asarray(seg_b, dtype=np.int64)
     lens = seg_b - seg_a
     rp = np.zeros(len(lens) + 1, dtype=np.uint64)
@@ -454,6 +482,31 @@ def _view(ptr, count, dtype):
     return np.ctypeslib.as_array(ctypes.cast(ptr, ctypes.POINTER(ctypes.c_uint8)), shape=(nbytes,)).view(dtype)
 
 
+def _read_result(tok, res, views, zero_copy=False):
+    """A b2t_result of tok's engine -> (numpy arrays, owner).  views(L, res) returns views of the result's pinned host
+    buffers (None for an array that was not asked for).  Without zero_copy the arrays are copies, the result is freed
+    and owner is None; with it they are the views themselves and owner is the _ResultOwner that frees the result:
+    whoever keeps the views must keep the owner."""
+    L = _lib.lib()
+    if zero_copy:
+        owner = _ResultOwner(res, tok)
+        return views(L, res), owner
+    try:
+        return tuple(None if a is None else a.copy() for a in views(L, res)), None
+    finally:
+        L.b2t_result_free(res)
+
+
+def _byte_span(data, a0, b0, o0, o1, byte_offsets):
+    """the byte span in data of a token with offsets (o0, o1) in the document data[a0:b0]; char offsets count the
+    document's UTF-8 lead bytes"""
+    if byte_offsets:
+        return a0 + o0, a0 + o1
+    lead = np.flatnonzero((data[a0:b0] & 0xC0) != 0x80)
+    at = lambda o: a0 + int(lead[o]) if o < lead.size else b0
+    return at(o0), at(o1)
+
+
 class Tokenizer:
     def __init__(self, tokenizer_json, device=-1):
         js = json.loads(tokenizer_json) if isinstance(tokenizer_json, (str, bytes)) else tokenizer_json
@@ -484,9 +537,9 @@ class Tokenizer:
         cfg = self._cfg
         L = _lib.lib()
         toks = list(self._vocab.keys())
-        vb, vo = _pack(toks)
+        vb, vo = _pack(toks, np.uint32)
         vi = np.fromiter((self._vocab[t] for t in toks), dtype=np.uint32, count=len(toks))
-        mb, mo = _pack([s for ab in cfg["merges"] for s in ab])
+        mb, mo = _pack([s for ab in cfg["merges"] for s in ab], np.uint32)
         c = _lib.Config()
         c.struct_size = ctypes.sizeof(_lib.Config)
         c.model, c.pretok = cfg["model"], cfg["pretok"]
@@ -517,7 +570,7 @@ class Tokenizer:
         if not toks:
             L.b2t_engine_set_added_tokens(self._h, 0, None, None, None, None)
             return
-        tb, to = _pack([t.content for t in toks])
+        tb, to = _pack([t.content for t in toks], np.uint32)
         ti = np.asarray([t.id for t in toks], dtype=np.uint32)
         tf = np.asarray([(_lib.ADDED_SINGLE_WORD if t.single_word else 0) | (_lib.ADDED_LSTRIP if t.lstrip else 0) |
                          (_lib.ADDED_RSTRIP if t.rstrip else 0) | (_lib.ADDED_NORMALIZED if t.normalized else 0) for t in toks], dtype=np.uint8)
@@ -560,12 +613,7 @@ class Tokenizer:
         return v
 
     def num_special_tokens_to_add(self, is_pair):
-        """PostProcessor::added_tokens (template.rs:647-653, bert.rs, roberta.rs)"""
-        tp = self._template
-        if tp is None:
-            return 0
-        pieces = tp["pair"] if is_pair else tp["single"]
-        return sum(1 for p in (pieces or []) if p[0] == "special")
+        return special_token_count(self._template, is_pair)
 
     def _add(self, tokens, special):
         """AddedVocabulary::add_tokens (added_vocabulary.rs:270-340): a token keeps the model's id when its content is in the
@@ -629,26 +677,23 @@ class Tokenizer:
 
     # ---- encode
     def _engine_rows(self, data, row_off, flags, zero_copy=False):
-        """The C-ABI call: packed rows in host memory -> row CSR (ids, offsets or None, word ids or None, row_ptr).
-        zero_copy: the arrays are views of the result's pinned buffers; `self._last_owner` keeps the result alive and the
-        caller ties it to whatever holds the views."""
+        """The C-ABI call: packed rows in host memory -> _Rows (ids, offsets or None, word ids or None, row_ptr): copies,
+        or with zero_copy views of the result whose _ResultOwner is the _Rows' `owner`."""
         n_rows = len(row_off) - 1
         L = _lib.lib()
         res = ctypes.c_void_p()
         _lib.check(L.b2t_encode_batch(self._h, data.ctypes.data if data.size else None, row_off.ctypes.data, n_rows, flags, ctypes.byref(res)))
-        owner = _ResultOwner(res) if zero_copy else None
-        try:
+
+        def views(L, res):
             T = L.b2t_result_n_tokens(res)
-            keep = (lambda a: a) if zero_copy else (lambda a: a.copy())
-            ids = keep(_view(L.b2t_result_ids(res), T, np.uint32))
-            offs = keep(_view(L.b2t_result_offsets(res), 2 * T, np.uint32).reshape(-1, 2)) if flags & _lib.WANT_OFFSETS else None
-            wid = keep(_view(L.b2t_result_word_ids(res), T, np.uint32)) if flags & _lib.WANT_WORD_IDS else None
-            rp = keep(_view(L.b2t_result_row_ptr(res), n_rows + 1, np.uint64))
-        finally:
-            if not zero_copy:
-                L.b2t_result_free(res)
-        self._last_owner = owner
-        return ids, offs, wid, rp
+            return (_view(L.b2t_result_ids(res), T, np.uint32),
+                    _view(L.b2t_result_offsets(res), 2 * T, np.uint32).reshape(-1, 2) if flags & _lib.WANT_OFFSETS else None,
+                    _view(L.b2t_result_word_ids(res), T, np.uint32) if flags & _lib.WANT_WORD_IDS else None,
+                    _view(L.b2t_result_row_ptr(res), n_rows + 1, np.uint64))
+        arrays, owner = _read_result(self, res, views, zero_copy)
+        rows = _Rows(arrays)
+        rows.owner = owner
+        return rows
 
     # ---- truncation / padding (bindings/python/src/tokenizer.rs:700-820)
     def enable_truncation(self, max_length, stride=0, strategy="longest_first", direction="right"):
@@ -676,60 +721,65 @@ class Tokenizer:
     def padding(self):
         return None if self._padding is None else dict(self._padding)
 
-    def _encode_core(self, data, doc_off, flags, raw, extract_added_tokens):
-        """added-token extraction -> engine -> stitching.  -> (BatchEncoding of the plain sequences, trim counts or None)"""
-        parts, cut, row_off, added_at, done = None, False, doc_off, [], False
-        tp = self._template
-        if extract_added_tokens and self._added is not None and self._dev_added:
-            # the extraction runs on the device; added tokens come back marked (bit 31 of the id).  Their matched spans are
-            # read off the offsets where the host needs the text (lstrip / rstrip tokens, offset trimming)
-            want_trim = tp is not None and tp["trim"] is not None and bool(flags & _lib.WANT_OFFSETS)
-            need_text = self._added_strip or want_trim
-            fl = flags | _lib.FLAG_ADDED_IDS | (_lib.WANT_OFFSETS if need_text else 0)
+    def _encode_core(self, data, doc_off, flags, extract_added_tokens, zero_copy=False):
+        """added-token extraction -> engine -> stitching.  -> (BatchEncoding of the plain sequences, trim counts or None);
+        with zero_copy the BatchEncoding's arrays may be views of the engine's result, kept valid by its `_owner`"""
+        if extract_added_tokens and self._dev_added:
             try:
-                ids, offs, wid, rp = self._engine_rows(data, doc_off, fl, getattr(self, "_zero_copy", False))
-                done = True
+                return self._encode_device_extraction(data, doc_off, flags, zero_copy)
             except _lib.B2TError as ex:
                 if ex.code != _lib.B2T_ERR_UNSUPPORTED:
-                    raise                     # (spans outside the device limits: split on the host below)
-            if done:
-                marked = np.flatnonzero(ids >> 31)
-                ids &= np.uint32(0x7FFFFFFF)
-                if need_text and marked.size:
-                    docs_of = np.searchsorted(rp, marked, side="right") - 1
-                    byte_off = bool(flags & _lib.OFFSETS_BYTES)
-                    for i, d in zip(marked.tolist(), docs_of.tolist()):
-                        a0, b0 = int(doc_off[d]), int(doc_off[d + 1])
-                        o0, o1 = int(offs[i, 0]), int(offs[i, 1])
-                        if byte_off:
-                            a, b = a0 + o0, a0 + o1
-                        else:   # characters -> bytes inside the document
-                            lead_pos = np.flatnonzero((data[a0:b0] & 0xC0) != 0x80)
-                            a = a0 + (int(lead_pos[o0]) if o0 < lead_pos.size else b0 - a0)
-                            b = a0 + (int(lead_pos[o1]) if o1 < lead_pos.size else b0 - a0)
-                        added_at.append((i, a, b))
-                if not (flags & _lib.WANT_OFFSETS):
-                    offs = None
-        if not done:
-            if extract_added_tokens and self._added is not None:
-                row_off, parts, cut = added.split_batch(self._added, raw, doc_off)
-            ids, offs, wid, rp = self._engine_rows(data, row_off, flags | (_lib.NO_ADDED_TOKENS if self._added is not None else 0), getattr(self, "_zero_copy", False))
-            if cut:
-                ids, offs, wid, rp, added_at = added.stitch_rows(raw, doc_off, parts, ids, offs, wid, rp, bool(flags & _lib.OFFSETS_BYTES))
+                    raise  # (spans outside the device limits: split on the host instead)
+        return self._encode_host_extraction(data, doc_off, flags, extract_added_tokens, zero_copy)
+
+    def _encode_device_extraction(self, data, doc_off, flags, zero_copy):
+        """The extraction runs on the device; added tokens come back marked (bit 31 of the id).  Their matched spans are
+        read off the offsets where the host needs the text (lstrip / rstrip tokens, offset trimming)."""
+        tp = self._template
+        need_text = self._added_strip or (tp is not None and tp["trim"] is not None and bool(flags & _lib.WANT_OFFSETS))
+        fl = flags | _lib.FLAG_ADDED_IDS | (_lib.WANT_OFFSETS if need_text else 0)
+        rows = self._engine_rows(data, doc_off, fl, zero_copy)
+        ids, offs, wid, rp = rows
+        marked = np.flatnonzero(ids >> 31)
+        ids &= np.uint32(0x7FFFFFFF)
+        added_at = []
+        if need_text and marked.size:
+            docs_of = np.searchsorted(rp, marked, side="right") - 1
+            for i, d in zip(marked.tolist(), docs_of.tolist()):
+                added_at.append((i, *_byte_span(data, int(doc_off[d]), int(doc_off[d + 1]), int(offs[i, 0]), int(offs[i, 1]),
+                                                 bool(flags & _lib.OFFSETS_BYTES))))
+        return self._plain_encoding(data, ids, offs if flags & _lib.WANT_OFFSETS else None, wid, rp, added_at, rows)
+
+    def _encode_host_extraction(self, data, doc_off, flags, extract_added_tokens, zero_copy):
+        """added.py cuts the documents at the added tokens, the engine encodes the pieces, and the rows are stitched back."""
+        row_off, parts, cut, added_at = doc_off, None, False, []
+        if extract_added_tokens and self._added is not None:
+            row_off, parts, cut = added.split_batch(self._added, data, doc_off)
+        rows = self._engine_rows(data, row_off, flags | (_lib.NO_ADDED_TOKENS if self._added is not None else 0), zero_copy)
+        ids, offs, wid, rp = rows
+        if cut:
+            ids, offs, wid, rp, added_at = added.stitch_rows(data, doc_off, parts, ids, offs, wid, rp, bool(flags & _lib.OFFSETS_BYTES))
+        return self._plain_encoding(data, ids, offs, wid, rp, added_at, rows)
+
+    def _plain_encoding(self, data, ids, offs, wid, rp, added_at, rows):
+        """-> (BatchEncoding, trim counts or None).  added_at: (token index, byte span in data) of the added tokens whose
+        matched text the host needs; rows: what _engine_rows returned, whose owner the BatchEncoding keeps."""
+        tp = self._template
         trim = None
         if tp is not None and tp["trim"] is not None and offs is not None:
             lead, trail = self._trim_tables()
             ld, tr = lead[ids], trail[ids]
             for i, a, b in added_at:
-                ld[i], tr[i] = self._span_spaces(raw, a, b)
+                ld[i], tr[i] = self._span_spaces(data, a, b)
             trim = (ld, tr)
         be = BatchEncoding(ids, offs, wid, rp)
+        be._owner = getattr(rows, "owner", None)   # (a replacement of the engine seam may return a plain tuple)
         for i, a, b in added_at:  # Token::new(id, value = the matched span): differs from the content after lstrip / rstrip
             tok = self._added.tokens[int(ids[i])]
             if b - a != len(tok.content.encode("utf-8")):
                 if be.token_text is None:
                     be.token_text = {}
-                be.token_text[i] = bytes(raw[a:b]).decode("utf-8", "replace")
+                be.token_text[i] = bytes(data[a:b]).decode("utf-8", "replace")
         return be, trim
 
     def _finish(self, be, trim, add_special_tokens):
@@ -757,14 +807,9 @@ class Tokenizer:
         data = np.ascontiguousarray(data, dtype=np.uint8)
         doc_off = np.ascontiguousarray(doc_off, dtype=np.uint64)
         flags = (_lib.WANT_OFFSETS if offsets else 0) | (_lib.WANT_WORD_IDS if word_ids else 0) | (_lib.OFFSETS_BYTES if byte_offsets else 0)
-        self._zero_copy = bool(zero_copy)
-        try:
-            be, trim = self._encode_core(data, doc_off, flags, data, extract_added_tokens)
-        finally:
-            self._zero_copy = False
+        be, trim = self._encode_core(data, doc_off, flags, extract_added_tokens, bool(zero_copy))
         out = self._finish(be, trim, add_special_tokens)
-        out._owner = getattr(self, "_last_owner", None) if zero_copy else None   # the views die with the BatchEncoding
-        self._last_owner = None
+        out._owner = be._owner   # the views die with the BatchEncoding
         return out
 
     # ---- dense mode: template + truncation + padding on the device (include/b2t.h b2t_encode_batch_dense)
@@ -796,11 +841,7 @@ class Tokenizer:
         with the tokenizer's truncation, template and padding applied on the device (what `encode_batch` + stacking the
         Encodings' ids / attention_mask gives in the reference).  `data` is a list of str, or packed (np.uint8[N], np.uint64[n+1])."""
         if doc_off is None:
-            bs = [d.encode("utf-8") for d in data]
-            doc_off = np.zeros(len(bs) + 1, dtype=np.uint64)
-            if bs:
-                np.cumsum([len(b) for b in bs], out=doc_off[1:])
-            data = np.frombuffer(b"".join(bs), dtype=np.uint8)
+            data, doc_off = _pack(data, np.uint64)
         data = np.ascontiguousarray(data, dtype=np.uint8)
         doc_off = np.ascontiguousarray(doc_off, dtype=np.uint64)
         if self._added is not None and not self._dev_added and added.split_batch(self._added, data, doc_off)[2]:
@@ -810,14 +851,14 @@ class Tokenizer:
         L = _lib.lib()
         res = ctypes.c_void_p()
         _lib.check(L.b2t_encode_batch_dense(self._h, data.ctypes.data if data.size else None, doc_off.ctypes.data, n, ctypes.byref(sp), ctypes.byref(res)))
-        try:
-            W = L.b2t_result_dense_length(res)
-            ids = _view(L.b2t_result_dense_ids(res), n * W, np.uint32).reshape(n, W).copy()
-            mask = _view(L.b2t_result_attention_mask(res), n * W, np.uint8).reshape(n, W).copy() if want_mask else None
-            lens = _view(L.b2t_result_row_lengths(res), n, np.uint32).copy()
-        finally:
-            L.b2t_result_free(res)
         del keep
+
+        def views(L, res):
+            W = L.b2t_result_dense_length(res)
+            return (_view(L.b2t_result_dense_ids(res), n * W, np.uint32).reshape(n, W),
+                    _view(L.b2t_result_attention_mask(res), n * W, np.uint8).reshape(n, W) if want_mask else None,
+                    _view(L.b2t_result_row_lengths(res), n, np.uint32))
+        (ids, mask, lens), _ = _read_result(self, res, views)
         return {"input_ids": ids, "attention_mask": mask, "lengths": lens}
 
     def _trim_tables(self):
@@ -855,6 +896,7 @@ class Tokenizer:
         """Batches with pairs of sequences: the engine encodes every sequence as a row of its own; truncation, the
         post-processor and the merge of the two halves (with all combinations of their overflowing parts) follow the
         reference one input at a time (pairs.py)."""
+        from . import pairs  # (pairs.py uses the post-processing rules of this module)
         seqs, first = [], []
         for x in inputs:
             first.append(len(seqs))
@@ -865,12 +907,8 @@ class Tokenizer:
             else:
                 raise UnsupportedConfig("inputs must be str or a pair (str, str)")
         first.append(len(seqs))
-        bs = [d.encode("utf-8") for d in seqs]
-        joined = b"".join(bs)
-        off = np.zeros(len(bs) + 1, dtype=np.uint64)
-        if bs:
-            np.cumsum(np.fromiter(map(len, bs), dtype=np.int64, count=len(bs)), out=off[1:])
-        be, trim = self._encode_core(np.frombuffer(joined, dtype=np.uint8), off, _lib.WANT_OFFSETS | _lib.WANT_WORD_IDS, joined, True)
+        data, off = _pack(seqs, np.uint64)
+        be, trim = self._encode_core(data, off, _lib.WANT_OFFSETS | _lib.WANT_WORD_IDS, True)
         rp = be.row_ptr.tolist()
         ids, offs, wid = be.ids.tolist(), [tuple(o) for o in be.offsets.tolist()], be.word_ids.tolist()
         ld, tr = (trim[0].tolist(), trim[1].tolist()) if trim is not None else (None, None)
@@ -917,20 +955,14 @@ class Tokenizer:
             # pre-tokenizer, model), its tokens keep offsets relative to the word and all get the word's index
             if any(isinstance(d, str) for d in docs):
                 raise TypeError("is_pretokenized=True expects sequences of words (List[str]), not str")
-            seq_rows = np.zeros(len(docs) + 1, dtype=np.int64)
-            if docs:
-                np.cumsum(np.fromiter(map(len, docs), dtype=np.int64, count=len(docs)), out=seq_rows[1:])
+            seq_rows = np.cumsum([0] + [len(d) for d in docs], dtype=np.int64)
             docs = [w for d in docs for w in d]
         try:
-            bs = [d.encode("utf-8") for d in docs]
+            data, off = _pack(docs, np.uint64)
         except AttributeError:
             raise UnsupportedConfig("only raw sequences (str), or lists of words with is_pretokenized=True, are supported; pairs are not") from None
-        joined = b"".join(bs)
-        off = np.zeros(len(bs) + 1, dtype=np.uint64)
-        if bs:
-            np.cumsum(np.fromiter(map(len, bs), dtype=np.int64, count=len(bs)), out=off[1:])
         flags = (_lib.WANT_OFFSETS if offsets else 0) | (_lib.WANT_WORD_IDS if word_ids else 0)
-        be, trim = self._encode_core(np.frombuffer(joined, dtype=np.uint8), off, flags, joined, True)
+        be, trim = self._encode_core(data, off, flags, True)
         if seq_rows is not None:  # rows (words) -> sequences
             wid = None
             if be.word_ids is not None:
@@ -944,13 +976,10 @@ class Tokenizer:
         part_doc = np.arange(len(be.row_ptr) - 1, dtype=np.int64)
         tr = self._truncation
         if tr is not None:
-            tp = self._template
-            n_added = len(tp["pre"]) + len(tp["post"]) if (add_special_tokens and tp is not None) else 0
-            if tr["max_length"] < n_added:
-                raise ValueError("truncation max_length is smaller than the number of special tokens the post-processor adds")
-            if tr["strategy"] == "only_second" and np.any(np.diff(be.row_ptr).astype(np.int64) > tr["max_length"] - n_added):
+            max_len = truncation_budget(tr, self._template, False, add_special_tokens)
+            if tr["strategy"] == "only_second" and np.any(np.diff(be.row_ptr).astype(np.int64) > max_len):
                 raise ValueError("Truncation error: Second sequence not provided")
-            be, cut, part_doc = truncate_csr(be, list(trim) if trim is not None else [], tr["max_length"] - n_added, tr["stride"], tr["direction"])
+            be, cut, part_doc = truncate_csr(be, list(trim) if trim is not None else [], max_len, tr["stride"], tr["direction"])
             trim = tuple(cut) if trim is not None else None
         be = self._finish(be, trim, add_special_tokens)
         rp = be.row_ptr.tolist()
@@ -1021,18 +1050,11 @@ class Tokenizer:
 
     def pre_tokenize_batch(self, docs):
         """PreTokenizer seam: per document the list of (start_byte, end_byte) of its splits."""
-        bs = [d.encode("utf-8") for d in docs]
-        off = np.zeros(len(bs) + 1, dtype=np.uint64)
-        if bs:
-            np.cumsum(np.fromiter(map(len, bs), dtype=np.int64, count=len(bs)), out=off[1:])
-        data = np.frombuffer(b"".join(bs), dtype=np.uint8)
+        data, off = _pack(docs, np.uint64)
+        n = len(off) - 1
         L = _lib.lib()
         res = ctypes.c_void_p()
-        _lib.check(L.b2t_pre_tokenize_batch(self._h, data.ctypes.data if data.size else None, off.ctypes.data, len(bs), ctypes.byref(res)))
-        try:
-            T = L.b2t_result_n_tokens(res)
-            offs = _view(L.b2t_result_offsets(res), 2 * T, np.uint32).reshape(-1, 2).copy()
-            rp = _view(L.b2t_result_row_ptr(res), len(bs) + 1, np.uint64).copy()
-        finally:
-            L.b2t_result_free(res)
-        return [[tuple(x) for x in offs[int(rp[i]):int(rp[i + 1])].tolist()] for i in range(len(bs))]
+        _lib.check(L.b2t_pre_tokenize_batch(self._h, data.ctypes.data if data.size else None, off.ctypes.data, n, ctypes.byref(res)))
+        (offs, rp), _ = _read_result(self, res, lambda L, res: (_view(L.b2t_result_offsets(res), 2 * L.b2t_result_n_tokens(res), np.uint32).reshape(-1, 2),
+                                                          _view(L.b2t_result_row_ptr(res), n + 1, np.uint64)))
+        return [[tuple(x) for x in offs[int(rp[i]):int(rp[i + 1])].tolist()] for i in range(n)]
