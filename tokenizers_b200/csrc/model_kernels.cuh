@@ -191,8 +191,11 @@ __device__ __forceinline__ bool wc_lookup(const ModelParams& P, const uint8_t* s
     if (q0.z != ~key.k[0] || q0.w != ~key.k[1]) continue;
     const uint4 q1 = ld_relaxed_v4(q + 1);
     if (q1.x != ~key.k[2] || q1.y != ~key.k[3] || q1.z != ~key.k[4] || q1.w != ~key.k[5]) continue;
-    const uint4 q2 = ld_relaxed_v4(q + 2), q3 = ld_relaxed_v4(q + 3);
+    const uint4 q2 = ld_relaxed_v4(q + 2);
     const int ntok = (int)(q2.x & 0xFFu);
+    // ids 2..5 only for words that have them (most have one or two tokens): the look-ups pay per L2 request, not per
+    // byte -- on an H100 at 700 W, one more load per look-up (the key together with the tag, same sector) cost bpe_tile 10 %
+    const uint4 q3 = ntok > 2 ? ld_relaxed_v4(q + 3) : make_uint4(0u, 0u, 0u, 0u);
     const uint32_t cids[6] = {q2.z, q2.w, q3.x, q3.y, q3.z, q3.w};   // complemented ids
     const uint32_t lens[6] = {(q2.x >> 8) & 0xFFu, (q2.x >> 16) & 0xFFu, q2.x >> 24, q2.y & 0xFFu, (q2.y >> 8) & 0xFFu, (q2.y >> 16) & 0xFFu};
     bool ok = ntok != 0 && (q2.y & WC_LEN_MARK);
