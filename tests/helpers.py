@@ -344,6 +344,68 @@ def scale_base(name, seed=0, n_corpus=600, n_fuzz=600):
     return pack_docs(docs)
 
 
+# ---------------------------------------------------------------------------------------------- page-edge placement
+PAGE = 2048
+EDGES = [0, 32, 256, 416, 1024]
+DELTAS = [-40, -33, -32, -31, -17, -16, -9, -8, -4, -3, -2, -1, 0, 1, 2, 3, 4, 8, 9, 16, 17, 31, 32, 33, 40]
+FILLER = b"lorem ipsum dolor sit amet, consectetur adipiscing elit "
+
+
+def place(slots, form, measure=lambda s: len(s.encode("utf-8"))):
+    """slots: [(probe, position, anchor)] with position increasing -> documents: the probe's start ("start") or end
+    ("end") lands at `position`, counted with `measure` (bytes of the batch the kernels see)"""
+    docs, text, pos = [], [], 0
+    for probe, p, anchor in slots:
+        a = p if anchor == "start" else p - measure(probe)
+        gap = a - pos
+        assert gap >= 0, (probe, p, anchor)
+        fill = (FILLER * (gap // len(FILLER) + 1))[:gap].decode()
+        if gap:
+            fill = fill[:-1] + "\n"
+        if form == "doc":
+            docs += [fill, probe]
+        else:
+            text.append(fill + probe)
+            if len(text) == 16:
+                docs.append("".join(text)); text = []
+        pos = a + measure(probe)
+    if text:
+        docs.append("".join(text))
+    return docs
+
+
+def page_slots(probes, deltas=DELTAS):
+    slots, k = [], 1
+    for probe in probes:
+        for e in EDGES:
+            for anchor in ("start", "end"):
+                for d in deltas:
+                    slots.append((probe, k * PAGE + e + d, anchor))
+                    k += 1
+    return slots
+
+
+_exp = {}
+
+
+def check(tj, docs, what, wcache=(True, False), byte_offsets=True):
+    """the engine against the oracle on `docs` (char offsets, and byte offsets when asked), word cache on and off"""
+    from oracle import oracle as orc
+    o = orc.Oracle(tj)
+    data, off = pack_docs(docs)
+    key = (tj, what)
+    if key not in _exp:
+        _exp[key] = (o.encode_batch_csr(data, off), o.encode_batch_csr(data, off, orc.OFF_BYTE) if byte_offsets else None)
+    exp_c, exp_b = _exp[key]
+    for wc in wcache:
+        tok = tokenizer_with_env(tj, B2T_WCACHE="1" if wc else "0")
+        be = tok.encode_batch_csr(data, off)
+        assert_csr_equal((be.ids, be.offsets, be.word_ids, be.row_ptr), exp_c, docs, f"{what} wcache={wc}")
+        if exp_b is not None:
+            be = tok.encode_batch_csr(data, off, byte_offsets=True)
+            assert_csr_equal((be.ids, be.offsets, be.word_ids, be.row_ptr), exp_b, docs, f"{what} byte offsets wcache={wc}")
+
+
 def added_token_docs(seed, n):
     """fuzz documents with the added tokens spliced in: glued to words, surrounded by spaces, back to back, truncated"""
     import random

@@ -16,11 +16,8 @@ pytestmark = pytest.mark.gpu
 
 from tokenizers_b200 import Tokenizer, _lib  # noqa: E402
 from oracle import oracle as orc  # noqa: E402
+from helpers import PAGE, DELTAS, place, page_slots, check  # noqa: E402
 
-PAGE = 2048
-EDGES = [0, 32, 256, 416, 1024]
-DELTAS = [-40, -33, -32, -31, -17, -16, -9, -8, -4, -3, -2, -1, 0, 1, 2, 3, 4, 8, 9, 16, 17, 31, 32, 33, 40]
-FILLER = b"lorem ipsum dolor sit amet, consectetur adipiscing elit "
 WIDE = {1: "abcdefghij", 2: "éßжяλ", 3: "中文語あア", 4: "𝒜𝒷𝓬𐐀𐐨"}   # letters (\p{L}) of 1..4 bytes
 
 
@@ -66,40 +63,6 @@ def wordpiece_probes(max_chars):
 BERT_PROBES = ["".join(chr(0xAC00 + (37 * i) % 11172) for i in range(k)) for k in (5, 40, 90)] + ["中文字" * 12, "x中y", "ÀÉÎÕÜ" * 8, "ǅİ"]
 
 
-def place(slots, form, measure=lambda s: len(s.encode("utf-8"))):
-    """slots: [(probe, position, anchor)] with position increasing -> documents: the probe's start ("start") or end
-    ("end") lands at `position`, counted with `measure` (bytes of the batch the kernels see)"""
-    docs, text, pos = [], [], 0
-    for probe, p, anchor in slots:
-        a = p if anchor == "start" else p - measure(probe)
-        gap = a - pos
-        assert gap >= 0, (probe, p, anchor)
-        fill = (FILLER * (gap // len(FILLER) + 1))[:gap].decode()
-        if gap:
-            fill = fill[:-1] + "\n"
-        if form == "doc":
-            docs += [fill, probe]
-        else:
-            text.append(fill + probe)
-            if len(text) == 16:
-                docs.append("".join(text)); text = []
-        pos = a + measure(probe)
-    if text:
-        docs.append("".join(text))
-    return docs
-
-
-def page_slots(probes, deltas=DELTAS):
-    slots, k = [], 1
-    for probe in probes:
-        for e in EDGES:
-            for anchor in ("start", "end"):
-                for d in deltas:
-                    slots.append((probe, k * PAGE + e + d, anchor))
-                    k += 1
-    return slots
-
-
 def scan_block_slots(probes):
     """around the 2 MiB boundaries of the page and tile scans (1024 pages): one probe per boundary"""
     rng = random.Random(3)
@@ -107,25 +70,6 @@ def scan_block_slots(probes):
     for m, probe in enumerate(probes, start=1):
         out.append((probe, m * (2 << 20) + rng.choice([-2, -1, 0, 1, 2]), rng.choice(["start", "end"])))
     return out
-
-
-_exp = {}
-
-
-def check(tj, docs, what, wcache=(True, False), byte_offsets=True):
-    o = orc.Oracle(tj)
-    data, off = helpers.pack_docs(docs)
-    key = (tj, what)
-    if key not in _exp:
-        _exp[key] = (o.encode_batch_csr(data, off), o.encode_batch_csr(data, off, orc.OFF_BYTE) if byte_offsets else None)
-    exp_c, exp_b = _exp[key]
-    for wc in wcache:
-        tok = helpers.tokenizer_with_env(tj, B2T_WCACHE="1" if wc else "0")
-        be = tok.encode_batch_csr(data, off)
-        helpers.assert_csr_equal((be.ids, be.offsets, be.word_ids, be.row_ptr), exp_c, docs, f"{what} wcache={wc}")
-        if exp_b is not None:
-            be = tok.encode_batch_csr(data, off, byte_offsets=True)
-            helpers.assert_csr_equal((be.ids, be.offsets, be.word_ids, be.row_ptr), exp_b, docs, f"{what} byte offsets wcache={wc}")
 
 
 @pytest.mark.parametrize("form", ["doc", "text"])

@@ -233,7 +233,8 @@ __global__ void __launch_bounds__(LONG_THREADS) bpe_long_kernel(const uint8_t* _
     uint32_t* aux = pool.aux + d.pool_off;
     uint4* out = pool.out + d.pool_off;
 
-    // whole pre-token in the vocabulary (ignore_merges)?  Only tokens up to 255 bytes are in the table.
+    // whole pre-token in the vocabulary (ignore_merges)?  The table holds every token, whatever its length (pieces of a
+    // cut pre-token are never looked up).
     if (tid == 0) s_hit = 0;
     __syncthreads();
     if (t.ignore_merges && !d.soft && L < 65536 && tid == 0) {
