@@ -367,12 +367,12 @@ static void launch_pretok(b2t_engine* e, const uint8_t* d_bytes, int64_t n, Work
   if constexpr (KIND == PT_LLAMA3) {
     if (added)
       pretok_stream_kernel<KIND, true><<<(unsigned)grid, K1_THREADS, 0, st>>>(d_bytes, n, ws.doc_bits.as<uint32_t>(), e->d_cls.as<uint32_t>(),
-                                                                            ws.start_bits.as<uint32_t>(), ws.drop_bits.as<uint32_t>(),
-                                                                            ws.page_sum.as<uint64_t>(), (int)n_kb, (int)kb, ab);
+                                                                            ws.start_bits.as<uint32_t>(), ws.page_sum.as<uint64_t>(),
+                                                                            (int)n_kb, (int)kb, ab);
     else
       pretok_stream_kernel<KIND><<<(unsigned)grid, K1_THREADS, 0, st>>>(d_bytes, n, ws.doc_bits.as<uint32_t>(), e->d_cls.as<uint32_t>(),
-                                                                      ws.start_bits.as<uint32_t>(), ws.drop_bits.as<uint32_t>(),
-                                                                      ws.page_sum.as<uint64_t>(), (int)n_kb, (int)kb);
+                                                                      ws.start_bits.as<uint32_t>(), ws.page_sum.as<uint64_t>(),
+                                                                      (int)n_kb, (int)kb);
   } else {
     const SwapMasks masks{0x55555555u, 0x33333333u, 0x0F0F0F0Fu};
     if (added)

@@ -5,7 +5,7 @@
 //   bytes      u8 [n]                input, read once by K1 with 16-byte loads
 //   doc_bits   u32[n/32 + 2]         bit p set <=> some document starts at byte p (K0; bit n is the end sentinel)
 //   start_bits u32[n/32 + 2]         bit p set <=> a pre-token (split) starts at byte p            (K1 output)
-//   drop_bits  u32[n/32 + 2]         Whitespace only: the split starting at p is removed whitespace (K1 output)
+//   drop_bits  u32[n/32 + 2]         Whitespace / Bert: the split starting at p is removed whitespace (K1 output)
 //   page_sum   u64[n/2048 + 1]       per 2 KB page: #chars, #kept splits, and the same counted from the last doc start
 //   page_carry u64[n/2048 + 1]       K1b: #chars (low 32) / #kept splits (high 32) of the document that spans into the
 //                                    page, counted from that document's start to the page start
@@ -17,12 +17,6 @@
 #include "pretok_logic.cuh"
 
 namespace b2t {
-
-struct ByteAtGlobal {
-  const uint8_t* __restrict__ p;
-  int64_t n;
-  __device__ __forceinline__ uint32_t operator()(int64_t i) const { return (i >= 0 && i < n) ? (uint32_t)__ldg(p + i) : 0u; }
-};
 
 // ------------------------------------------------------------------------------------------------ K0
 // One thread per document boundary d in [0, n_docs]: marks the doc start bit and fills page_first_doc.
@@ -37,47 +31,7 @@ __global__ void doc_mark_kernel(const uint64_t* __restrict__ doc_off, uint32_t n
   for (uint64_t p = p_lo; p <= p_hi; ++p) page_first_doc[p] = d;
 }
 
-// ------------------------------------------------------------------------------------------------ K1
-__device__ __forceinline__ void load_chunk_words(const uint8_t* __restrict__ bytes, int64_t base, int64_t n, uint32_t w[8]) {
-  if (base + CHUNK <= n) {
-    const uint4* q = reinterpret_cast<const uint4*>(bytes + base);
-    uint4 a = __ldg(q), b = __ldg(q + 1);
-    w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
-  } else {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      uint32_t x = 0;
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        int64_t p = base + j * 4 + k;
-        if (p < n) x |= (uint32_t)__ldg(bytes + p) << (8 * k);
-      }
-      w[j] = x;
-    }
-  }
-}
-
-template <int KIND>
-__device__ __forceinline__ ChunkMasks classify_global(const uint8_t* __restrict__ bytes, int64_t n, int64_t chunk,
-                                                      const uint32_t* __restrict__ cls_tbl) {
-  ChunkMasks m;
-  int64_t base = chunk * CHUNK;
-  if (chunk < 0 || base >= n) {
-    m.lead = m.L = m.N = m.S = m.SP = m.NL = m.AP = 0u;
-    return m;
-  }
-  uint32_t w[8];
-  load_chunk_words(bytes, base, n, w);
-  ByteAtGlobal at{bytes, n};
-  return classify_chunk(w, base, n, at, cls_tbl, KIND);
-}
-
-struct DsAtGlobal {
-  const uint32_t* __restrict__ doc_bits;
-  int64_t n_chunks;
-  __device__ __forceinline__ uint32_t operator()(int64_t k) const { return (k >= 0 && k < n_chunks) ? __ldg(doc_bits + k) : 0u; }
-};
-
+// ------------------------------------------------------------------------------------------------ K1 page summary
 // page summary packing: [11:0] chars, [23:12] kept splits, [35:24] chars since last doc start, [47:36] splits since, [48] has doc start
 __device__ __forceinline__ uint64_t pack_sum(uint32_t tot, uint32_t aft, uint32_t flag) {
   // tot / aft carry two 16-bit fields each (chars | splits << 16)
@@ -180,62 +134,40 @@ __global__ void __launch_bounds__(SCAN_BLOCK) page_scan_top_kernel(const uint64_
 // pretok_lean_kernel (GPT-2, Whitespace, Bert, no regex) and pretok_stream_kernel (Llama-3), one kernel per
 // pre-tokenizer with the same streaming structure.  Every WARP streams through its own contiguous range of the batch, 1 KB
 // (32 chunks of 32 bytes, one per lane) per iteration, and is independent of all other warps: no shared memory, no
-// block barrier.  Iteration i+1 is classified (pretok_fast.cuh: bit planes -> classes) before the boundaries of
+// block barrier.  Iteration i+1 is classified (pretok_logic.cuh: bit planes -> classes) before the boundaries of
 // iteration i are evaluated, so a lane gets everything it needs from its neighbours with warp shuffles:
 //   the chunk before lane 0   = lane 31 of the previous iteration (still in that lane's registers),
 //   the chunk after lane 31   = lane 0 of the next iteration (already classified).
 // The range ends are handled by classifying one extra KB on either side.  Page summaries (2 KB = two iterations of the
 // same warp) are combined in registers.  Algorithmic traffic is unchanged: 1.25 B per input byte.
-#include "pretok_fast.cuh"
-
+// Both kernels are built from the same steps (warp range, chunk load, valid mask, page summary); their loops stay
+// apart because their register budgets and pipelines differ: the lean kernel runs at 64 registers, the Llama-3 kernel
+// keeps two iterations of class masks live at 128.
 namespace b2t {
-
-// The Llama-3 slow path: the exact window code (pretok_logic.cuh) for one chunk whose runs reach beyond its window,
-// everything re-read from global memory and the carry walked over chunk masks re-classified from there.
-template <int KIND>
-__device__ __noinline__ uint32_t exact_chunk_start(const uint8_t* __restrict__ bytes, int64_t n, int64_t c,
-                                                  const uint32_t* __restrict__ cls_tbl, const uint32_t* __restrict__ doc_bits) {
-  static_assert(KIND == PT_LLAMA3, "the slow path of the Llama-3 kernel");
-  const int64_t n_chunks = n / CHUNK + 1;
-  ByteAtGlobal at{bytes, n};
-  DsAtGlobal dsat{doc_bits, n_chunks};
-  const ChunkMasks p = classify_global<KIND>(bytes, n, c - 1, cls_tbl), o = classify_global<KIND>(bytes, n, c, cls_tbl),
-                   x = classify_global<KIND>(bytes, n, c + 1, cls_tbl);
-  Window w;
-  w.lead = win(p.lead, o.lead, x.lead); w.L = win(p.L, o.L, x.L); w.N = win(p.N, o.N, x.N); w.S = win(p.S, o.S, x.S);
-  w.SP = win(p.SP, o.SP, x.SP); w.NL = win(p.NL, o.NL, x.NL); w.AP = win(p.AP, o.AP, x.AP);
-  w.DS = win(dsat(c - 1), dsat(c), dsat(c + 1));
-  const int64_t wb = c * CHUNK - 16;
-  struct GlobalMaskAt {
-    const uint8_t* bytes; int64_t n; const uint32_t* cls;
-    __device__ __forceinline__ ChunkMasks operator()(int64_t k) const { return classify_global<KIND>(bytes, n, k, cls); }
-  } masks{bytes, n, cls_tbl};
-  const LlamaCarry cy = llama_carry(c, n_chunks, masks, dsat);
-  return boundaries_llama3(w, wb, at, cy).start;
-}
 
 constexpr int K1_THREADS = 128;
 constexpr int K1_LEAN_MINBLOCKS = 8;
 constexpr int K1_WINDOW_MINBLOCKS = 4;   // window (Llama-3) form: more live state
 
-// byte access with 32-bit positions (batches are < 2^31 bytes; "negative" positions wrap to out-of-range)
-struct ByteAt32 {
-  const uint8_t* __restrict__ p;
-  uint32_t n;
-  __device__ __forceinline__ uint32_t operator()(uint32_t i) const { return i < n ? (uint32_t)__ldg(p + i) : 0u; }
-};
-// the four bytes at q..q+3 (q < n) as one word: two aligned loads and a funnel shift
-struct At4Global {
-  const uint32_t* __restrict__ words;
-  uint32_t n;
-  __device__ __forceinline__ uint32_t operator()(uint32_t q) const {
-    const uint32_t a0 = __ldg(words + (q >> 2)), a1 = ((q | 3u) + 1u < n) ? __ldg(words + (q >> 2) + 1) : 0u;
-    return __funnelshift_r(a0, a1, (q & 3u) * 8u);
-  }
-};
+// ---------------------------------------------------------------------------------------------- steps of both kernels
+// This warp's iterations [it_lo, it_hi); false when it has none.  it_lo is even: a page is two consecutive iterations
+// of one warp.
+__device__ __forceinline__ bool warp_range(int n_kb, int kb_per_warp, int& it_lo, int& it_hi) {
+  const int gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  it_lo = gw * kb_per_warp;
+  if (it_lo >= n_kb) return false;
+  it_hi = it_lo + kb_per_warp < n_kb ? it_lo + kb_per_warp : n_kb;
+  return true;
+}
 
-// the chunk that holds the end of the batch: aligned word loads, bytes at or past n masked off (stays in registers)
-__device__ __forceinline__ void load_tail_words(const uint8_t* __restrict__ bytes, uint32_t base, uint32_t n, uint32_t w[8]) {
+// the 32 bytes at p as little-endian words: two 16-byte loads
+__device__ __forceinline__ void load32(const uint8_t* p, uint32_t w[8]) {
+  const uint4* q = reinterpret_cast<const uint4*>(p);
+  const uint4 a = __ldg(q), b = __ldg(q + 1);
+  w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
+}
+// The chunk that holds the end of the batch: aligned word loads, bytes at or past n masked off.
+__device__ __forceinline__ void load_tail_words(const uint8_t* bytes, uint32_t base, uint32_t n, uint32_t w[8]) {
   const uint32_t* __restrict__ words = reinterpret_cast<const uint32_t*>(bytes + base);
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
@@ -248,6 +180,71 @@ __device__ __forceinline__ void load_tail_words(const uint8_t* __restrict__ byte
     w[j] = x;
   }
 }
+// load(it, w): the words of this lane's chunk of iteration `it` (it < 0: nothing there, all zero); bytes at or past n
+// read as 0.  (A functor rather than a function: nvcc then lays out the lean kernel exactly as with a local lambda.)
+struct ChunkLoader {
+  const uint8_t* __restrict__ bytes;
+  uint32_t n;
+  int lane;
+  __device__ __forceinline__ void operator()(int it, uint32_t w[8]) const {
+    const uint32_t base = ((uint32_t)it * 32u + lane) * CHUNK;
+    if (it >= 0 && base + CHUNK <= n) {
+      load32(bytes + base, w);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) w[j] = 0u;
+      if (it >= 0 && base < n) load_tail_words(bytes, base, n, w);
+    }
+  }
+};
+// the bytes of the chunk at `base` that lie inside the batch (none unless `there`)
+__device__ __forceinline__ uint32_t chunk_valid(bool there, uint32_t base, uint32_t n) {
+  return !there || base >= n ? 0u : (n - base >= CHUNK ? 0xFFFFFFFFu : (0xFFFFFFFFu >> (32u - (n - base))));
+}
+
+// The segmented page summary of a warp (counts restart at the last doc start of the page), built one iteration (half a
+// page) at a time: add() takes this lane's lead bytes, kept splits and document starts of iteration `it`, and lane 0
+// writes page_sum when the page is complete.  tot / aft / flag: the first half of the current page.
+struct PageSummary {
+  uint32_t tot, aft, flag;
+  __device__ __forceinline__ void add(int it, int n_kb, uint32_t n, int lane, uint32_t lead, uint32_t kept, uint32_t docw,
+                                      uint64_t* page_sum) {
+    constexpr unsigned FULL = 0xFFFFFFFFu;
+    const uint32_t t1 = (uint32_t)__popc(lead) | ((uint32_t)__popc(kept) << 16);
+    const unsigned dsm = __ballot_sync(FULL, docw != 0u);
+    const uint32_t wtot = __reduce_add_sync(FULL, t1);
+    uint32_t waft = 0u;
+    if (dsm) {
+      const int last = 31 - __clz((int)dsm);
+      uint32_t mine = 0u;
+      if (lane > last) mine = t1;
+      else if (lane == last) {
+        const uint32_t from = ~bits_below(31 - __clz((int)docw));
+        mine = (uint32_t)__popc(lead & from) | ((uint32_t)__popc(kept & from) << 16);
+      }
+      waft = __reduce_add_sync(FULL, mine);
+    }
+    const uint32_t wflag = dsm != 0u;
+    const uint32_t page = (uint32_t)it >> 1;
+    if (it & 1) {
+      const uint32_t a = wflag ? waft : aft + wtot, t = tot + wtot, f = flag | wflag;
+      if (lane == 0 && page * (uint32_t)PAGE <= n) page_sum[page] = pack_sum(t, a, f);
+    } else {
+      tot = wtot; aft = waft; flag = wflag;
+      if (it + 1 >= n_kb && lane == 0 && page * (uint32_t)PAGE <= n) page_sum[page] = pack_sum(tot, aft, flag);  // the batch ends in the first half
+    }
+  }
+};
+
+// the four bytes at q..q+3 (q < n) as one word: two aligned loads and a funnel shift
+struct At4Global {
+  const uint32_t* __restrict__ words;
+  uint32_t n;
+  __device__ __forceinline__ uint32_t operator()(uint32_t q) const {
+    const uint32_t a0 = __ldg(words + (q >> 2)), a1 = ((q | 3u) + 1u < n) ? __ldg(words + (q >> 2) + 1) : 0u;
+    return __funnelshift_r(a0, a1, (q & 3u) * 8u);
+  }
+};
 
 // ---------------------------------------------------------------------------------------------- lean form (GPT-2, Whitespace, no regex)
 // Stage A (iteration j): bit planes, classes, and all of the boundary algebra that looks backwards.  Stage B
@@ -265,34 +262,20 @@ pretok_lean_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint32_
                    uint64_t* __restrict__ page_sum, int n_kb, int kb_per_warp, SwapMasks masks, AddedBits ab = AddedBits{nullptr, nullptr, nullptr}) {
   constexpr unsigned FULL = 0xFFFFFFFFu;
   const int lane = threadIdx.x & 31;
-  const int gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int it_lo = gw * kb_per_warp;             // even: a page is two consecutive iterations of one warp
-  if (it_lo >= n_kb) return;
-  const int it_hi = it_lo + kb_per_warp < n_kb ? it_lo + kb_per_warp : n_kb;
+  int it_lo, it_hi;
+  if (!warp_range(n_kb, kb_per_warp, it_lo, it_hi)) return;
   const uint32_t n = (uint32_t)n64;
   const uint32_t n_chunks = n / CHUNK + 1;
   const At4Global at4{reinterpret_cast<const uint32_t*>(bytes), n};
   const int up = (lane + 31) & 31, down = (lane + 1) & 31;
-
-  auto load = [&](int it, uint32_t w[8]) {       // it = -1: nothing there
-    const uint32_t base = ((uint32_t)it * 32u + lane) * CHUNK;
-    if (it >= 0 && base + CHUNK <= n) {
-      const uint4* q = reinterpret_cast<const uint4*>(bytes + base);
-      const uint4 a = __ldg(q), b = __ldg(q + 1);
-      w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) w[j] = 0u;
-      if (it >= 0 && base < n) load_tail_words(bytes, base, n, w);
-    }
-  };
+  const ChunkLoader load{bytes, n, lane};   // load(it, w): it = -1: nothing there
 
   // carries of my chunk of the previous iteration (lane 31's chunk precedes lane 0's)
   uint32_t kL = 0u, kN = 0u, kS = 0u, kSP = 0u, k_ov = 0u;
   // stage A results of iteration j - 1, waiting for stage B
   uint32_t p_start = 0u, p_drop = 0u, p_lead = 0u, p_head = 0u, p_ds = 0u, p_dsn = 0u, p_s31 = 0u;
   uint32_t p_inner = 0u, p_doc = 0u;              // ADDED only
-  uint32_t h_tot = 0u, h_aft = 0u, h_flag = 0u;   // first half of the current page
+  PageSummary ps{0u, 0u, 0u};
 
   uint32_t w[8];
   load(it_lo > 0 ? it_lo - 1 : -1, w);
@@ -303,13 +286,11 @@ pretok_lean_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint32_
     // interior iteration (warp-uniform): this KB and the first chunk of the next one lie inside the batch
     const bool interior = j >= 0 && ((uint32_t)j * 32u + 33u) * CHUNK <= n;
     uint32_t valid = 0xFFFFFFFFu;
-    if (!interior) valid = j < 0 || base >= n ? 0u : (n - base >= CHUNK ? 0xFFFFFFFFu : (0xFFFFFFFFu >> (32u - (n - base))));
+    if (!interior) valid = chunk_valid(j >= 0, base, n);
     uint32_t b[8];
     bitslice32(w, b, masks);
     if (j + 1 < it_hi && ((uint32_t)j * 32u + 64u) * CHUNK <= n) {   // prefetch; the common case first: a whole KB inside the batch
-      const uint4* q = reinterpret_cast<const uint4*>(bytes + (uint32_t)(base + 32u * CHUNK));   // (j = -1: the sum wraps to lane * 32)
-      const uint4 a = __ldg(q), bq = __ldg(q + 1);
-      w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = bq.x; w[5] = bq.y; w[6] = bq.z; w[7] = bq.w;
+      load32(bytes + (uint32_t)(base + 32u * CHUNK), w);          // (j = -1: the sum wraps to lane * 32)
     } else {
       load(j + 1 <= it_hi ? j + 1 : -1, w);      // range / batch ends (the KB after the range is classified too, for its first bytes)
     }
@@ -339,7 +320,7 @@ pretok_lean_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint32_
     }
     uint32_t start, drop = 0u;
     if (KIND == PT_GPT2) {
-      const FastOut o = fast_gpt2(m, pt, 1u, 1u, ds, ds_next, base, at4);
+      const FastOut o = fast_gpt2(m, pt, ds, ds_next, base, at4);
       Overflow in; in.bits = __shfl_sync(FULL, lane == 31 ? k_ov : o.ov.bits, up);
       k_ov = o.ov.bits;
       start = apply_overflow(o.start, m.lead, in);
@@ -360,36 +341,11 @@ pretok_lean_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint32_
         fin = finalize_gpt2(fin, p_lead, p_s31, xh & 15u, xh >> 4, p_dsn);
       }
       if (ADDED) fin &= ~p_inner;      // an added token's span is one pre-token
-      const uint32_t p_docw = ADDED ? p_doc : p_ds;
       if (pc < n_chunks) {
         start_bits[pc] = fin;
         if (pretok_drops_whitespace(KIND)) drop_bits[pc] = p_drop;
       }
-      // ---- page summary (segmented: counts restart at the last doc start of the page); one iteration is half a page
-      const uint32_t kept = fin & ~p_drop;
-      const uint32_t tot = (uint32_t)__popc(p_lead) | ((uint32_t)__popc(kept) << 16);
-      const unsigned dsm = __ballot_sync(FULL, p_docw != 0u);
-      const uint32_t wtot = __reduce_add_sync(FULL, tot);
-      uint32_t waft = 0u;
-      if (dsm) {
-        const int last = 31 - __clz((int)dsm);
-        uint32_t mine = 0u;
-        if (lane > last) mine = tot;
-        else if (lane == last) {
-          const uint32_t from = ~bits_below(31 - __clz((int)p_docw));
-          mine = (uint32_t)__popc(p_lead & from) | ((uint32_t)__popc(kept & from) << 16);
-        }
-        waft = __reduce_add_sync(FULL, mine);
-      }
-      const uint32_t wflag = dsm != 0u;
-      const uint32_t page = (uint32_t)it >> 1;
-      if (it & 1) {
-        const uint32_t a = wflag ? waft : h_aft + wtot, t = h_tot + wtot, f = h_flag | wflag;
-        if (lane == 0 && page * (uint32_t)PAGE <= n) page_sum[page] = pack_sum(t, a, f);
-      } else {
-        h_tot = wtot; h_aft = waft; h_flag = wflag;
-        if (it + 1 >= n_kb && lane == 0 && page * (uint32_t)PAGE <= n) page_sum[page] = pack_sum(h_tot, h_aft, h_flag);  // the batch ends in the first half
-      }
+      ps.add(it, n_kb, n, lane, p_lead, fin & ~p_drop, ADDED ? p_doc : p_ds, page_sum);
     }
     p_start = start; p_drop = drop; p_lead = m.lead; p_head = head; p_ds = ds; p_dsn = ds_next; p_s31 = m.S >> 31;
     if (ADDED) { p_inner = inner; p_doc = docw; }
@@ -397,44 +353,52 @@ pretok_lean_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint32_
 }
 
 // ---------------------------------------------------------------------------------------------- window form (Llama-3)
-// Same streaming structure with the 64-bit window algebra of pretok_logic.cuh (two iterations per trip).  drop_bits is
-// not written: the tiktoken pattern removes nothing, every split is kept.
+// Same streaming structure with the 64-bit window algebra of pretok_logic.cuh (two iterations per trip).  Only
+// start_bits is written: the tiktoken pattern removes nothing, every split is kept.
+
+struct DsAtGlobal {
+  const uint32_t* __restrict__ doc_bits;
+  int64_t n_chunks;
+  __device__ __forceinline__ uint32_t operator()(int64_t k) const { return (k >= 0 && k < n_chunks) ? __ldg(doc_bits + k) : 0u; }
+};
+
+// The slow path for chunk c, whose window w has a run that reaches its edge.  Out of line, so that the hot loop's
+// registers do not change.  llama_carry walks the chunks around c, classified again from global memory.
+static __device__ __noinline__ uint32_t llama3_slow_start(Window w, const uint8_t* __restrict__ bytes, uint32_t n, uint32_t c,
+                                                          const uint32_t* __restrict__ cls_tbl, const uint32_t* __restrict__ rbits) {
+  const uint32_t n_chunks = n / CHUNK + 1;
+  const At4Global at4{reinterpret_cast<const uint32_t*>(bytes), n};
+  const auto masks = [&](int64_t k) {
+    uint32_t wk[8];
+    const uint32_t base = (uint32_t)k * CHUNK;
+    ChunkLoader{bytes, n, (int)(k & 31)}((int)(k >> 5), wk);   // chunk k = lane k % 32 of iteration k / 32
+    return classify_standalone<PT_LLAMA3>(wk, chunk_valid(true, base, n), base, at4, cls_tbl);
+  };
+  return llama3_slow_path(w, c, n_chunks, masks, DsAtGlobal{rbits, n_chunks}, at4);
+}
+
 template <int KIND, bool ADDED = false>
 __global__ void __launch_bounds__(K1_THREADS, K1_WINDOW_MINBLOCKS)
 pretok_stream_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint32_t* __restrict__ doc_bits,
-                     const uint32_t* __restrict__ cls_tbl, uint32_t* __restrict__ start_bits, uint32_t* __restrict__ drop_bits,
+                     const uint32_t* __restrict__ cls_tbl, uint32_t* __restrict__ start_bits,
                      uint64_t* __restrict__ page_sum, int n_kb, int kb_per_warp, AddedBits ab = AddedBits{nullptr, nullptr, nullptr}) {
+  static_assert(KIND == PT_LLAMA3, "the window form is the Llama-3 kernel");
   constexpr unsigned FULL = 0xFFFFFFFFu;
   const int lane = threadIdx.x & 31;
-  const int gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int it_lo = gw * kb_per_warp;             // even: a page is two consecutive iterations of one warp
-  if (it_lo >= n_kb) return;
-  const int it_hi = it_lo + kb_per_warp < n_kb ? it_lo + kb_per_warp : n_kb;
+  int it_lo, it_hi;
+  if (!warp_range(n_kb, kb_per_warp, it_lo, it_hi)) return;
   const uint32_t n = (uint32_t)n64;
   const uint32_t n_chunks = n / CHUNK + 1;
-  static_assert(KIND == PT_LLAMA3, "the window form is the Llama-3 kernel");
   const At4Global at4{reinterpret_cast<const uint32_t*>(bytes), n};
   const int up = (lane + 31) & 31, down = (lane + 1) & 31;
 
-  auto load = [&](int it, uint32_t w[8]) {       // it = -1: nothing there
-    const uint32_t base = ((uint32_t)it * 32u + lane) * CHUNK;
-    if (it >= 0 && base + CHUNK <= n) {
-      const uint4* q = reinterpret_cast<const uint4*>(bytes + base);
-      const uint4 a = __ldg(q), b = __ldg(q + 1);
-      w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) w[j] = 0u;
-      if (it >= 0 && base < n) load_tail_words(bytes, base, n, w);   // the batch ends inside this chunk
-    }
-  };
+  const ChunkLoader load{bytes, n, lane};   // it = -1: nothing there
   // classes of iteration `it`; `prev` = this lane's classes of the iteration before (lane 31's chunk precedes lane 0's)
   auto classify = [&](const uint32_t w[8], int it, const FastCls& prev, FastCls& m, FastCls& pm) {
     const uint32_t base = ((uint32_t)it * 32u + lane) * CHUNK;
-    const uint32_t valid = it < 0 || base >= n ? 0u : (n - base >= CHUNK ? 0xFFFFFFFFu : (0xFFFFFFFFu >> (32u - (n - base))));
     uint32_t b[8];
     bitslice32(w, b);
-    m = classify_planes<KIND>(b, valid);
+    m = classify_planes<KIND>(b, chunk_valid(it >= 0, base, n));
     if (__any_sync(FULL, m.hi != 0u)) {
       if (m.unc) resolve_uncertain(m, at4, base, cls_tbl);
       fill_own(m);
@@ -450,7 +414,7 @@ pretok_stream_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint3
     if (m.cont & 1u) spill_in(m, pm.L, pm.N, pm.S);
   };
 
-  uint32_t h_tot = 0u, h_aft = 0u, h_flag = 0u;   // first half of the current page
+  PageSummary ps{0u, 0u, 0u};
 
   // One iteration: classify it+1 (words in w) into nxt / pnxt, refill w with the words of it+3, then boundaries,
   // stores and page summary of iteration `it` (classes in cur / pcur).
@@ -465,7 +429,7 @@ pretok_stream_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint3
     const uint32_t docw = ADDED ? (c < n_chunks ? __ldg(doc_bits + c) : 0u) : ds;
     uint32_t start;
     {
-      // window algebra of pretok_logic.cuh on [16 B of the previous chunk | mine | 16 B of the next chunk]
+      // window algebra on [16 B of the previous chunk | mine | 16 B of the next chunk]
       Window wd;
       auto nextw = [&](uint32_t mine, uint32_t theirs) { return __shfl_sync(FULL, lane == 0 ? theirs : mine, down); };
       wd.lead = win(pcur.lead, cur.lead, nextw(cur.lead, nxt.lead)); wd.L = win(pcur.L, cur.L, nextw(cur.L, nxt.L));
@@ -475,37 +439,13 @@ pretok_stream_kernel(const uint8_t* __restrict__ bytes, int64_t n64, const uint3
       const uint32_t ds_prev = (c >= 1u && c - 1u < n_chunks) ? __ldg(rbits + c - 1) : 0u;
       wd.DS = win(ds_prev, ds, ds_next);
       LlamaCarry cy; cy.n_count_before_window = 0; cy.zone_before_window = false; cy.tail_after_window = false;
-      const ByteAtGlobal at64{bytes, n64};
-      const BoundaryOut r = boundaries_llama3(wd, (int64_t)base - 16, at64, cy);
+      const BoundaryOut r = boundaries_llama3(wd, (int64_t)base - 16, at4, cy);
       start = r.start;
-      if (r.slow) start = exact_chunk_start<KIND>(bytes, n64, c, cls_tbl, rbits);
+      if (r.slow) start = llama3_slow_start(wd, bytes, n, c, cls_tbl, rbits);
     }
     if (ADDED && c < n_chunks) start &= ~__ldg(ab.inner + c);   // an added token's span is one pre-token
     if (c < n_chunks) start_bits[c] = start;
-    // ---- page summary (segmented: counts restart at the last doc start of the page); this iteration is half a page
-    const uint32_t tot = (uint32_t)__popc(cur.lead) | ((uint32_t)__popc(start) << 16);
-    const unsigned dsm = __ballot_sync(FULL, docw != 0u);
-    const uint32_t wtot = __reduce_add_sync(FULL, tot);
-    uint32_t waft = 0u;
-    if (dsm) {
-      const int last = 31 - __clz((int)dsm);
-      uint32_t mine = 0u;
-      if (lane > last) mine = tot;
-      else if (lane == last) {
-        const uint32_t from = ~bits_below(31 - __clz((int)docw));
-        mine = (uint32_t)__popc(cur.lead & from) | ((uint32_t)__popc(start & from) << 16);
-      }
-      waft = __reduce_add_sync(FULL, mine);
-    }
-    const uint32_t wflag = dsm != 0u;
-    const uint32_t page = (uint32_t)it >> 1;
-    if (it & 1) {
-      const uint32_t a = wflag ? waft : h_aft + wtot, t = h_tot + wtot, f = h_flag | wflag;
-      if (lane == 0 && page * (uint32_t)PAGE <= n) page_sum[page] = pack_sum(t, a, f);
-    } else {
-      h_tot = wtot; h_aft = waft; h_flag = wflag;
-      if (it + 1 >= n_kb && lane == 0 && page * (uint32_t)PAGE <= n) page_sum[page] = pack_sum(h_tot, h_aft, h_flag);  // the batch ends in the first half
-    }
+    ps.add(it, n_kb, n, lane, cur.lead, start, docw, page_sum);
   };
 
   FastCls A, pA, B, pB;   // p*: the chunk before (as far as needed)
