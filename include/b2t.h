@@ -29,7 +29,8 @@ typedef enum {
   B2T_ERR_UNSUPPORTED = 2, /* configuration outside the hot path (the reference would handle it on CPU) */
   B2T_ERR_CUDA = 3,        /* CUDA runtime error, message has the details */
   B2T_ERR_VOCAB = 4,       /* merge token out of vocabulary / missing [UNK] (models/bpe/mod.rs:12-36, wordpiece/mod.rs:17-22) */
-  B2T_ERR_TOO_LARGE = 5    /* batch exceeds the per-call device limits */
+  B2T_ERR_TOO_LARGE = 5,   /* batch exceeds the per-call device limits */
+  B2T_ERR_TRUNCATION = 6   /* TruncationError::SequenceTooShort (utils/truncation.rs:155): a pair cannot be cut to max_length */
 } b2t_status;
 
 /* models::ModelWrapper variants on the path (models/mod.rs:60-68) */
@@ -92,7 +93,7 @@ enum { B2T_ADDED_SINGLE_WORD = 1u, B2T_ADDED_LSTRIP = 2u, B2T_ADDED_RSTRIP = 4u,
 
 /* Replaces TokenizerBuilder::build for the path.  The tables are uploaded to the device once; the engine is
  * immutable afterwards and may be used from several host threads: every host-buffer call (b2t_encode_batch,
- * b2t_encode_batch_dense, b2t_pre_tokenize_batch) runs on device workspaces and streams of its own (up to four calls in
+ * b2t_encode_batch_dense, b2t_encode_pairs_dense, b2t_pre_tokenize_batch) runs on device workspaces and streams of its own (up to four calls in
  * flight, further ones wait), so their copies and kernels overlap; the device-resident entry points share one workspace
  * (their result lives in it) and serialise.  With profiling on (b2t_engine_set_profiling) calls are meant to be made one at a time. */
 int b2t_engine_create(const b2t_config* cfg, b2t_engine** out);
@@ -171,6 +172,46 @@ uint32_t b2t_result_dense_length(const b2t_result* r);        /* L */
 const uint32_t* b2t_result_dense_ids(const b2t_result* r);    /* n_docs * L */
 const uint8_t* b2t_result_attention_mask(const b2t_result* r); /* n_docs * L, or NULL */
 const uint32_t* b2t_result_row_lengths(const b2t_result* r);  /* n_docs */
+
+/* Dense mode for PAIRS of sequences (EncodeInput::Dual): what the reference runs after the path for a batch of pairs --
+ * truncate_encodings with a pair (utils/truncation.rs:70-162, kept parts only), the pair template (processors/template.rs:
+ * 544-643 apply_template; BertProcessing / RobertaProcessing pair forms; default_process without a post-processor) and
+ * padding (utils/padding.rs:50-81), as TokenizerImpl::post_process orders them (tokenizer/mod.rs:1265-1317) -- done on the
+ * device.  The batch is 2 n_pairs documents: document 2p is the first sequence of pair p, 2p + 1 the second.  The result
+ * is n_pairs dense rows of ids, type ids (+ attention mask + row lengths); b2t_result_n_docs is n_pairs.  Overflowing parts
+ * (stride) are not part of a dense batch. */
+enum { B2T_TRUNC_LONGEST_FIRST = 0, B2T_TRUNC_ONLY_FIRST = 1, B2T_TRUNC_ONLY_SECOND = 2 };  /* TruncationStrategy */
+/* the sequence pieces of a template's piece list (token ids are < 2^20, so these never collide with one) */
+enum { B2T_PIECE_A = 0x80000000u, B2T_PIECE_B = 0x80000001u };
+typedef struct {
+  uint32_t struct_size;        /* sizeof(b2t_pair_dense_spec) */
+  uint32_t length;             /* PaddingStrategy::Fixed(length); 0 = BatchLongest (the batch in one device pass: < 2^31 bytes) */
+  uint32_t pad_to_multiple_of; /* PaddingParams.pad_to_multiple_of, 0 = none */
+  uint32_t max_length;         /* TruncationParams.max_length, special tokens included; 0 = no truncation */
+  int32_t strategy;            /* B2T_TRUNC_* */
+  int32_t truncate_left;       /* TruncationDirection::Left: keep the LAST tokens of each sequence */
+  uint32_t pad_id;             /* PaddingParams.pad_id */
+  uint32_t pad_type_id;        /* PaddingParams.pad_type_id (<= 255) */
+  int32_t pad_left;            /* PaddingDirection::Left */
+  /* the pair template (Template::pair, processors/template.rs): n_pieces entries, each a special token id or B2T_PIECE_A /
+   * B2T_PIECE_B (exactly one of each, in the template's order), with its type id (<= 255).  Without a post-processor:
+   * {A: 0, B: 1}; with add_special_tokens = false: the template's two sequence pieces only. At most 8 special tokens
+   * before, between and after the sequences. */
+  uint32_t n_pieces;
+  const uint32_t* piece_ids;
+  const uint32_t* piece_types;
+  uint32_t want_mask;          /* also return the attention mask (u8 per position); type ids and row lengths always come back */
+} b2t_pair_dense_spec;
+
+/* HOST buffers in (doc_off holds 2 n_pairs + 1 offsets), pinned host rows out.  A pair that cannot be truncated fails the
+ * batch with B2T_ERR_TRUNCATION; a row that does not fit a fixed length with B2T_ERR_INVALID (as b2t_encode_batch_dense). */
+int b2t_encode_pairs_dense(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_pairs,
+                           const b2t_pair_dense_spec* spec, b2t_result** out);
+/* Device buffers in (as b2t_encode_batch_device, 2 n_pairs + 1 offsets), device rows out (owned by the engine until the next call). */
+int b2t_encode_pairs_dense_device(b2t_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off,
+                                  uint32_t n_pairs, const b2t_pair_dense_spec* spec, void* stream, b2t_result** out);
+/* Encoding::get_type_ids of every row of a pair result: row p = type_ids[p * L .. (p + 1) * L); NULL for other results. */
+const uint8_t* b2t_result_type_ids(const b2t_result* r);
 
 /* Replaces PreTokenizer::pre_tokenize (tokenizer/mod.rs:65-67) for a batch: the splits of every document as
  * (start, end) BYTE offsets into the document (offsets[2k], offsets[2k+1]); row_ptr delimits documents.  ids and

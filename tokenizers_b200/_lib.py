@@ -4,18 +4,21 @@ import ctypes, os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B2T_LIB") or os.path.join(_HERE, "libb2t.so")  # B2T_LIB: developer override for A/B builds
 
-B2T_OK, B2T_ERR_INVALID, B2T_ERR_UNSUPPORTED, B2T_ERR_CUDA, B2T_ERR_VOCAB, B2T_ERR_TOO_LARGE = range(6)
+B2T_OK, B2T_ERR_INVALID, B2T_ERR_UNSUPPORTED, B2T_ERR_CUDA, B2T_ERR_VOCAB, B2T_ERR_TOO_LARGE, B2T_ERR_TRUNCATION = range(7)
 MODEL_BPE, MODEL_WORDPIECE = 0, 1
 PRETOK_BYTELEVEL, PRETOK_LLAMA3, PRETOK_WHITESPACE, PRETOK_BYTELEVEL_NOREGEX, PRETOK_BERT = 0, 1, 2, 3, 4
 NORM_BERT, NORM_CLEAN_TEXT, NORM_CHINESE_CHARS, NORM_STRIP_ACCENTS, NORM_LOWERCASE = 0x100, 1, 2, 4, 8
 WANT_OFFSETS, WANT_WORD_IDS, OFFSETS_BYTES, NO_ADDED_TOKENS, FLAG_ADDED_IDS = 1, 2, 4, 8, 16
 ADDED_SINGLE_WORD, ADDED_LSTRIP, ADDED_RSTRIP, ADDED_NORMALIZED = 1, 2, 4, 8
+TRUNC_LONGEST_FIRST, TRUNC_ONLY_FIRST, TRUNC_ONLY_SECOND = 0, 1, 2
+PIECE_A, PIECE_B = 0x80000000, 0x80000001
 
 # every symbol include/b2t.h declares
 SYMBOLS = ["b2t_engine_create", "b2t_engine_destroy", "b2t_engine_set_added_tokens", "b2t_encode_batch", "b2t_encode_batch_device", "b2t_encode_batch_device_begin",
            "b2t_encode_batch_device_finish", "b2t_pre_tokenize_batch",
            "b2t_encode_batch_dense", "b2t_encode_batch_dense_device", "b2t_result_dense_length", "b2t_result_dense_ids",
            "b2t_result_attention_mask", "b2t_result_row_lengths",
+           "b2t_encode_pairs_dense", "b2t_encode_pairs_dense_device", "b2t_result_type_ids",
            "b2t_result_n_tokens", "b2t_result_n_docs", "b2t_result_on_device", "b2t_result_ids", "b2t_result_offsets",
            "b2t_result_word_ids", "b2t_result_row_ptr", "b2t_result_free", "b2t_host_alloc", "b2t_host_free",
            "b2t_engine_set_profiling", "b2t_engine_last_kernels", "b2t_unicode_class_table", "b2t_bert_normalizer_images", "b2t_last_error", "b2t_version"]
@@ -35,6 +38,14 @@ class DenseSpec(ctypes.Structure):
     _fields_ = [("struct_size", ctypes.c_uint32), ("length", ctypes.c_uint32), ("pad_to_multiple_of", ctypes.c_uint32),
                 ("max_length", ctypes.c_uint32), ("pad_id", ctypes.c_uint32), ("truncate_left", ctypes.c_int32), ("pad_left", ctypes.c_int32),
                 ("n_pre", ctypes.c_uint32), ("n_post", ctypes.c_uint32), ("pre_ids", ctypes.c_void_p), ("post_ids", ctypes.c_void_p),
+                ("want_mask", ctypes.c_uint32)]
+
+
+class PairDenseSpec(ctypes.Structure):
+    _fields_ = [("struct_size", ctypes.c_uint32), ("length", ctypes.c_uint32), ("pad_to_multiple_of", ctypes.c_uint32),
+                ("max_length", ctypes.c_uint32), ("strategy", ctypes.c_int32), ("truncate_left", ctypes.c_int32),
+                ("pad_id", ctypes.c_uint32), ("pad_type_id", ctypes.c_uint32), ("pad_left", ctypes.c_int32),
+                ("n_pieces", ctypes.c_uint32), ("piece_ids", ctypes.c_void_p), ("piece_types", ctypes.c_void_p),
                 ("want_mask", ctypes.c_uint32)]
 
 
@@ -68,7 +79,9 @@ def lib():
     L.b2t_encode_batch_dense.argtypes = [vp, vp, vp, u32, ctypes.POINTER(DenseSpec), ctypes.POINTER(vp)]
     L.b2t_encode_batch_dense_device.argtypes = [vp, vp, u64, vp, u32, ctypes.POINTER(DenseSpec), vp, ctypes.POINTER(vp)]
     L.b2t_result_dense_length.argtypes = [vp]; L.b2t_result_dense_length.restype = u32
-    for f in ("b2t_result_dense_ids", "b2t_result_attention_mask", "b2t_result_row_lengths"):
+    L.b2t_encode_pairs_dense.argtypes = [vp, vp, vp, u32, ctypes.POINTER(PairDenseSpec), ctypes.POINTER(vp)]
+    L.b2t_encode_pairs_dense_device.argtypes = [vp, vp, u64, vp, u32, ctypes.POINTER(PairDenseSpec), vp, ctypes.POINTER(vp)]
+    for f in ("b2t_result_dense_ids", "b2t_result_attention_mask", "b2t_result_row_lengths", "b2t_result_type_ids"):
         getattr(L, f).argtypes = [vp]; getattr(L, f).restype = vp
     L.b2t_result_n_tokens.argtypes = [vp]; L.b2t_result_n_tokens.restype = u64
     L.b2t_result_n_docs.argtypes = [vp]; L.b2t_result_n_docs.restype = u32

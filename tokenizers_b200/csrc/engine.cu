@@ -119,12 +119,17 @@ struct PinBuf {
   template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
-// Dense mode request (b2t_encode_batch_dense*): the device-side spec plus how L is chosen.
+// Dense mode request (b2t_encode_batch_dense*, b2t_encode_pairs_dense*): the device-side spec plus how L is chosen.
 struct DenseReq {
-  DenseSpec S;
+  DenseSpec S;                  // single sequences (docs_per_row 1)
+  PairDenseSpec P;              // pairs (docs_per_row 2): documents 2p and 2p + 1 make row p
+  uint32_t docs_per_row = 1;
   bool batch_longest = false;   // padding strategy BatchLongest: L = longest row of the batch (after pad_to_multiple_of)
   uint32_t multiple = 0;        // pad_to_multiple_of
   bool want_mask = false;
+  bool pairs() const { return docs_per_row == 2; }
+  uint32_t& L() { return pairs() ? P.L : S.L; }
+  uint32_t L() const { return pairs() ? P.L : S.L; }
 };
 
 // How far run_device_pipeline goes: pre-tokenization only (K0..K1b), up to the token count (the caller finishes into its
@@ -156,7 +161,7 @@ struct Workspace {
   DevBuf page_long, long_desc, long_desc1, soft_bits, page_soft, lp_id, lp_val, lp_len, lp_plen, lp_aux, lp_out;  // long BPE pre-tokens (long_kernels.cuh)
   unsigned long long pool_cap = 0;
   DevBuf wcache;                      // per-batch word cache (model_kernels.cuh)
-  DevBuf dense_ids, dense_mask, dense_len;  // dense [n_docs, L] rows (dense_kernels.cuh)
+  DevBuf dense_ids, dense_mask, dense_len, dense_type;  // dense [n_rows, L] rows (dense_kernels.cuh); type ids: pairs only
   // BertNormalizer pre-pass (norm_kernels.cuh): the normalized batch and what maps its tokens back to the original
   DevBuf nrm_doc_bits, nrm_pfd, nrm_page_out, nrm_page_chars, nrm_lexcl_o, nrm_bsum_o, nrm_lexcl_c, nrm_bsum_c, nrm_tot, nrm_bytes, nrm_src_char, nrm_doc_off, nrm_doc_char0;
   bool norm_active = false;
@@ -179,10 +184,12 @@ struct b2t_result {
   uint64_t n_tokens = 0;
   const uint32_t* ids = nullptr; const uint32_t* offsets = nullptr; const uint32_t* word_ids = nullptr; const uint64_t* row_ptr = nullptr;
   PinBuf h_ids, h_offsets, h_word_ids, h_row_ptr;  // host results own pinned memory (returned to the engine pool on free)
-  // dense mode (b2t_encode_batch_dense*): [n_docs, dense_len] rows instead of the CSR
+  // dense mode (b2t_encode_batch_dense*, b2t_encode_pairs_dense*): [n_docs, dense_len] rows instead of the CSR (n_docs =
+  // pairs for a pair result, which also has type ids)
   uint32_t dense_len = 0;
   const uint32_t* dense_ids = nullptr; const uint8_t* dense_mask = nullptr; const uint32_t* row_len = nullptr;
-  PinBuf h_dense_ids, h_dense_mask, h_row_len;
+  const uint8_t* type_ids = nullptr;
+  PinBuf h_dense_ids, h_dense_mask, h_row_len, h_type_ids;
 };
 
 constexpr int NSLOT = 3;   // chunk workspaces of one host-path call: NSLOT - 1 chunks are in flight while the next is issued
@@ -422,17 +429,68 @@ static int make_dense_req(const b2t_dense_spec* sp, DenseReq* dq) {
   dq->want_mask = sp->want_mask != 0;
   return B2T_OK;
 }
+// b2t_pair_dense_spec -> DenseReq (pairs), checked: the piece list is split into pre X mid Y post
+static int make_dense_req(const b2t_pair_dense_spec* sp, DenseReq* dq) {
+  if (!sp) return fail(B2T_ERR_INVALID, "pair dense spec is null");
+  if (sp->struct_size != sizeof(b2t_pair_dense_spec))
+    return fail(B2T_ERR_INVALID, "b2t_pair_dense_spec: struct_size mismatch (%u != %zu)", sp->struct_size, sizeof(b2t_pair_dense_spec));
+  if (sp->n_pieces && (!sp->piece_ids || !sp->piece_types)) return fail(B2T_ERR_INVALID, "pair dense spec: null piece list");
+  if (sp->strategy < B2T_TRUNC_LONGEST_FIRST || sp->strategy > B2T_TRUNC_ONLY_SECOND) return fail(B2T_ERR_INVALID, "unknown truncation strategy %d", sp->strategy);
+  if (sp->pad_type_id > 255) return fail(B2T_ERR_UNSUPPORTED, "pad type id %u: type ids above 255 are not supported", sp->pad_type_id);
+  PairDenseSpec& P = dq->P;
+  memset(&P, 0, sizeof(P));
+  uint32_t n_seg[3] = {0, 0, 0}, seg = 0, n_a = 0, n_b = 0;
+  for (uint32_t i = 0; i < sp->n_pieces; ++i) {
+    const uint32_t id = sp->piece_ids[i], ty = sp->piece_types[i];
+    if (ty > 255) return fail(B2T_ERR_UNSUPPORTED, "template type id %u: type ids above 255 are not supported", ty);
+    if (id == B2T_PIECE_A || id == B2T_PIECE_B) {
+      const bool x = seg == 0;   // the first sequence piece is X
+      if (id == B2T_PIECE_A) ++n_a; else ++n_b;
+      if (x) P.b_first = id == B2T_PIECE_B;
+      (x ? P.type_x : P.type_y) = ty;
+      ++seg;
+      continue;
+    }
+    if (id >= (1u << 20)) return fail(B2T_ERR_UNSUPPORTED, "template token id %u: ids of 2^20 and above are not supported", id);
+    if (seg > 2 || n_seg[seg] >= (uint32_t)DENSE_MAX_SPECIAL)
+      return fail(B2T_ERR_UNSUPPORTED, "pair templates with more than %d special tokens before, between or after the sequences are not supported", DENSE_MAX_SPECIAL);
+    P.special[seg * DENSE_MAX_SPECIAL + n_seg[seg]++] = id | ty << 24;
+  }
+  if (n_a != 1 || n_b != 1) return fail(B2T_ERR_INVALID, "a pair template holds sequence A and sequence B exactly once each");
+  // pre, mid, post back to back, as the kernel indexes them
+  for (uint32_t i = 0; i < n_seg[1]; ++i) P.special[n_seg[0] + i] = P.special[DENSE_MAX_SPECIAL + i];
+  for (uint32_t i = 0; i < n_seg[2]; ++i) P.special[n_seg[0] + n_seg[1] + i] = P.special[2 * DENSE_MAX_SPECIAL + i];
+  P.n_pre = n_seg[0]; P.n_mid = n_seg[1]; P.n_post = n_seg[2];
+  const uint32_t n_special = P.n_pre + P.n_mid + P.n_post;
+  // tokenizer/mod.rs:1272-1283: the pair is truncated to max_length - n_added_tokens
+  if (sp->max_length && sp->max_length < n_special) return fail(B2T_ERR_INVALID, "max_length %u is smaller than the %u special tokens of the template", sp->max_length, n_special);
+  P.budget = sp->max_length ? sp->max_length - n_special : DENSE_NO_LIMIT;
+  P.strategy = (uint32_t)sp->strategy;
+  P.pad_id = sp->pad_id; P.pad_type = sp->pad_type_id;
+  P.trunc_left = sp->truncate_left ? 1 : 0; P.pad_left = sp->pad_left ? 1 : 0;
+  dq->docs_per_row = 2;
+  dq->batch_longest = sp->length == 0;
+  dq->multiple = sp->pad_to_multiple_of;
+  P.L = dq->batch_longest ? 0u : dense_round(sp->length, dq->multiple);
+  dq->want_mask = sp->want_mask != 0;
+  return B2T_OK;
+}
 
-// CSR of the workspace -> dense rows in ws.dense_* (asynchronous on st)
-static int launch_dense(b2t_engine* e, Workspace& ws, uint32_t n_docs, const DenseReq& dq, cudaStream_t st) {
+// CSR of the workspace -> dense rows in ws.dense_* (asynchronous on st); n_rows = documents / docs_per_row
+static int launch_dense(b2t_engine* e, Workspace& ws, uint32_t n_rows, const DenseReq& dq, cudaStream_t st) {
   int rc;
-  const size_t cells = (size_t)n_docs * dq.S.L;
-  if ((rc = ws.dense_ids.ensure(cells * 4 + 16)) || (rc = ws.dense_len.ensure((size_t)n_docs * 4 + 16)) ||
-      (dq.want_mask && (rc = ws.dense_mask.ensure(cells + 16))))
+  const size_t cells = (size_t)n_rows * dq.L();
+  if ((rc = ws.dense_ids.ensure(cells * 4 + 16)) || (rc = ws.dense_len.ensure((size_t)n_rows * 4 + 16)) ||
+      (dq.want_mask && (rc = ws.dense_mask.ensure(cells + 16))) || (dq.pairs() && (rc = ws.dense_type.ensure(cells + 16))))
     return rc;
-  if (n_docs && dq.S.L)
-    dense_rows_kernel<<<(unsigned)(((uint64_t)n_docs * 32 + 255) / 256), 256, 0, st>>>(
-        ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_docs, dq.S, ws.dense_ids.as<uint32_t>(),
+  const unsigned grid = (unsigned)(((uint64_t)n_rows * 32 + 255) / 256);
+  if (n_rows && dq.L() && dq.pairs())
+    dense_pair_rows_kernel<<<grid, 256, 0, st>>>(ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.P, ws.dense_ids.as<uint32_t>(),
+                                                 ws.dense_type.as<uint8_t>(), dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr,
+                                                 ws.dense_len.as<uint32_t>());
+  else if (n_rows && dq.L())
+    dense_rows_kernel<<<grid, 256, 0, st>>>(
+        ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.S, ws.dense_ids.as<uint32_t>(),
         dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr, ws.dense_len.as<uint32_t>(), nullptr);
   e->last_launches++;
   CU(cudaGetLastError());
@@ -685,10 +743,16 @@ static int finish_tail(b2t_engine* e, Workspace& ws, cudaStream_t st) {
   rec(e, st, "scan_compact");
   if (dq && finish) {
     ctl_block* ctl = ws.ctl.as<ctl_block>();
-    if (n_docs) row_len_max_kernel<<<(n_docs + 255) / 256, 256, 0, st>>>(ws.row_ptr.as<uint64_t>(), n_docs, dq->S.keep_max, dq->S.n_pre + dq->S.n_post, &ctl->max_row);
+    const uint32_t n_rows = n_docs / dq->docs_per_row;
+    const PairDenseSpec& P = dq->P;
+    if (n_rows && dq->pairs())
+      pair_len_max_kernel<<<(n_rows + 255) / 256, 256, 0, st>>>(ws.row_ptr.as<uint64_t>(), n_rows, P.budget, P.strategy, P.n_pre + P.n_mid + P.n_post,
+                                                              &ctl->max_row, &ctl->err);
+    else if (n_rows)
+      row_len_max_kernel<<<(n_rows + 255) / 256, 256, 0, st>>>(ws.row_ptr.as<uint64_t>(), n_rows, dq->S.keep_max, dq->S.n_pre + dq->S.n_post, &ctl->max_row);
     e->last_launches++;
-    if (!dq->batch_longest && (rc = launch_dense(e, ws, n_docs, *dq, st))) return rc;
-    rec(e, st, "dense_rows");
+    if (!dq->batch_longest && (rc = launch_dense(e, ws, n_rows, *dq, st))) return rc;
+    rec(e, st, dq->pairs() ? "dense_pair_rows" : "dense_rows");
   }
   CU(cudaMemcpyAsync(ws.h_ctl.p, ws.ctl.p, sizeof(ctl_block), cudaMemcpyDeviceToHost, st));
   return B2T_OK;
@@ -727,7 +791,10 @@ static int check_run(b2t_engine* e, Workspace& ws, cudaStream_t st, bool* reran 
       return fail(B2T_ERR_UNSUPPORTED, "added-token extraction: a span over %d bytes, more spans than one per 16 input bytes, or overlapping spans; "
                   "pass B2T_NO_ADDED_TOKENS and split on the host", ADDED_MAX_SPAN);
     if ((c->err | c->lc.err) & ERR_INTERNAL) return fail(B2T_ERR_CUDA, "internal error: long pre-token / added-token bookkeeping mismatch");
-    if (!(c->lc.err & ERR_POOL_OVERFLOW)) return B2T_OK;
+    if (!(c->lc.err & ERR_POOL_OVERFLOW)) {
+      if (c->err & ERR_TRUNCATION) return fail(B2T_ERR_TRUNCATION, "Truncation error: Sequence to truncate too short to respect the provided max_length");
+      return B2T_OK;
+    }
     if (attempt >= 2) return fail(B2T_ERR_CUDA, "long pool did not converge");
     if (reran) *reran = true;
     int rc;
@@ -765,12 +832,15 @@ extern "C" int b2t_engine_last_kernels(const b2t_engine* e, const char** names, 
   return e->last_launches;
 }
 
-// The device-resident entry points: argument checks (and in dense mode the spec, read into *dq), then the whole call under
-// dev_mu on the engine's one device workspace, on the caller's stream or the engine's own.  `done(ws, st)` takes the
-// finished run after the host has waited for it.
-template <class Done>
+// the spec argument of the entry points that are not dense
+static const b2t_dense_spec* const NO_SPEC = nullptr;
+
+// The device-resident entry points: argument checks (and in dense mode the spec -- b2t_dense_spec or b2t_pair_dense_spec --
+// read into *dq), then the whole call under dev_mu on the engine's one device workspace, on the caller's stream or the
+// engine's own.  `done(ws, st)` takes the finished run after the host has waited for it.
+template <class Spec, class Done>
 static int device_encode(const char* fn, b2t_engine* e, const void* out, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off,
-                         uint32_t n_docs, uint32_t flags, RunUntil until, const b2t_dense_spec* spec, DenseReq* dq, void* stream, Done&& done) {
+                         uint32_t n_docs, uint32_t flags, RunUntil until, const Spec* spec, DenseReq* dq, void* stream, Done&& done) {
   if (!e || !out || !d_doc_off || (!d_bytes && n_bytes)) return fail(B2T_ERR_INVALID, "%s: null argument", fn);
   if (((uintptr_t)d_bytes & 15u) != 0) return fail(B2T_ERR_INVALID, "%s: d_bytes must be 16-byte aligned", fn);
   int rc;
@@ -789,7 +859,7 @@ static int device_encode(const char* fn, b2t_engine* e, const void* out, const u
 
 extern "C" int b2t_encode_batch_device(b2t_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off,
                                        uint32_t n_docs, uint32_t flags, void* stream, b2t_result** out) {
-  return device_encode("b2t_encode_batch_device", e, out, d_bytes, n_bytes, d_doc_off, n_docs, flags, RUN_RESULT, nullptr, nullptr, stream,
+  return device_encode("b2t_encode_batch_device", e, out, d_bytes, n_bytes, d_doc_off, n_docs, flags, RUN_RESULT, NO_SPEC, nullptr, stream,
                        [&](Workspace& ws, cudaStream_t) -> int {
     b2t_result* r = new b2t_result();
     r->eng = e; r->on_device = 1; r->n_docs = n_docs;
@@ -805,7 +875,7 @@ extern "C" int b2t_encode_batch_device(b2t_engine* e, const uint8_t* d_bytes, ui
 
 extern "C" int b2t_encode_batch_device_begin(b2t_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off,
                                              uint32_t n_docs, uint32_t flags, void* stream, uint64_t* n_tokens) {
-  return device_encode("b2t_encode_batch_device_begin", e, n_tokens, d_bytes, n_bytes, d_doc_off, n_docs, flags, RUN_COUNT, nullptr, nullptr, stream,
+  return device_encode("b2t_encode_batch_device_begin", e, n_tokens, d_bytes, n_bytes, d_doc_off, n_docs, flags, RUN_COUNT, NO_SPEC, nullptr, stream,
                        [&](Workspace& ws, cudaStream_t) -> int {
     *n_tokens = ws.h_ctl.as<ctl_block>()->total;
     ws.pending = true;
@@ -895,34 +965,57 @@ extern "C" int b2t_engine_set_added_tokens(b2t_engine* e, uint32_t n_tokens, con
 extern "C" int b2t_encode_batch_dense(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, const b2t_dense_spec* spec,
                                       b2t_result** out);
 
-extern "C" int b2t_encode_batch_dense_device(b2t_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off, uint32_t n_docs,
-                                             const b2t_dense_spec* spec, void* stream, b2t_result** out) {
+// the dense device entry points: the rows of n_rows rows (n_docs / dq.docs_per_row) after the run
+template <class Spec>
+static int dense_device(const char* fn, b2t_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off, uint32_t n_docs,
+                        const Spec* spec, void* stream, b2t_result** out) {
   DenseReq dq;
-  return device_encode("b2t_encode_batch_dense_device", e, out, d_bytes, n_bytes, d_doc_off, n_docs, 0u, RUN_RESULT, spec, &dq, stream,
+  return device_encode(fn, e, out, d_bytes, n_bytes, d_doc_off, n_docs, 0u, RUN_RESULT, spec, &dq, stream,
                        [&](Workspace& ws, cudaStream_t st) -> int {
     int rc2;
-    const uint32_t max_row = ws.h_ctl.as<ctl_block>()->max_row;
+    const uint32_t max_row = ws.h_ctl.as<ctl_block>()->max_row, n_rows = n_docs / dq.docs_per_row;
     if (dq.batch_longest) {
-      dq.S.L = dense_round(max_row, dq.multiple);
-      if ((rc2 = launch_dense(e, ws, n_docs, dq, st))) return rc2;   // asynchronous on st, like the CSR entry point's result
-    } else if (max_row > dq.S.L) {
-      return fail(B2T_ERR_INVALID, "a row of %u tokens does not fit the dense length %u: enable truncation (the reference returns a longer row here)", max_row, dq.S.L);
+      dq.L() = dense_round(max_row, dq.multiple);
+      if ((rc2 = launch_dense(e, ws, n_rows, dq, st))) return rc2;   // asynchronous on st, like the CSR entry point's result
+    } else if (max_row > dq.L()) {
+      return fail(B2T_ERR_INVALID, "a row of %u tokens does not fit the dense length %u: enable truncation (the reference returns a longer row here)", max_row, dq.L());
     }
     b2t_result* r = new b2t_result();
-    r->eng = e; r->on_device = 1; r->n_docs = n_docs;
+    r->eng = e; r->on_device = 1; r->n_docs = n_rows;
     r->n_tokens = ws.h_ctl.as<ctl_block>()->total;
-    r->dense_len = dq.S.L;
+    r->dense_len = dq.L();
     r->dense_ids = ws.dense_ids.as<uint32_t>(); r->row_len = ws.dense_len.as<uint32_t>();
     r->dense_mask = dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr;
+    r->type_ids = dq.pairs() ? ws.dense_type.as<uint8_t>() : nullptr;
     *out = r;
     return B2T_OK;
   });
 }
 
+extern "C" int b2t_encode_batch_dense_device(b2t_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off, uint32_t n_docs,
+                                             const b2t_dense_spec* spec, void* stream, b2t_result** out) {
+  return dense_device("b2t_encode_batch_dense_device", e, d_bytes, n_bytes, d_doc_off, n_docs, spec, stream, out);
+}
+
+// a batch of n_pairs pairs is a batch of 2 n_pairs documents
+static int pair_docs(const char* fn, uint32_t n_pairs, uint32_t* n_docs) {
+  if (n_pairs > UINT32_MAX / 2) return fail(B2T_ERR_TOO_LARGE, "%s: %u pairs are more than 2^32 - 1 documents", fn, n_pairs);
+  *n_docs = 2 * n_pairs;
+  return B2T_OK;
+}
+
+// Replaces TokenizerImpl::post_process for a batch of pairs (tokenizer/mod.rs:1265-1317), see include/b2t.h
+extern "C" int b2t_encode_pairs_dense_device(b2t_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off, uint32_t n_pairs,
+                                             const b2t_pair_dense_spec* spec, void* stream, b2t_result** out) {
+  uint32_t n_docs = 0;
+  int rc = pair_docs("b2t_encode_pairs_dense_device", n_pairs, &n_docs);
+  return rc ? rc : dense_device("b2t_encode_pairs_dense_device", e, d_bytes, n_bytes, d_doc_off, n_docs, spec, stream, out);
+}
+
 // ------------------------------------------------------------------------------------------------ host pipeline
 static b2t_result* pool_get(b2t_engine* e) {
   std::lock_guard<std::mutex> lk(e->mu);
-  if (!e->pool.empty()) { b2t_result* r = e->pool.back().release(); e->pool.pop_back(); return r; }
+  if (!e->pool.empty()) { b2t_result* r = e->pool.back().release(); e->pool.pop_back(); r->type_ids = nullptr; return r; }
   return new b2t_result();
 }
 
@@ -964,14 +1057,15 @@ __global__ void rebase_kernel(uint64_t* doc_off, uint32_t count, uint64_t base) 
 
 struct Chunk { uint32_t d0, d1; uint64_t b0, b1; uint64_t tok_base; };
 
-// Queues the copy of a chunk's dense rows (documents d0 .. d0 + nd - 1) into the pinned result, on the slot's stream.
-static int queue_dense_copy(b2t_result* r, const Workspace& ws, uint32_t d0, uint32_t nd, const DenseReq& dq) {
-  const size_t L = dq.S.L;
-  if (nd && L) {
-    CU(cudaMemcpyAsync(r->h_dense_ids.as<uint32_t>() + (size_t)d0 * L, ws.dense_ids.p, (size_t)nd * L * 4, cudaMemcpyDeviceToHost, ws.stream));
-    if (dq.want_mask) CU(cudaMemcpyAsync(r->h_dense_mask.as<uint8_t>() + (size_t)d0 * L, ws.dense_mask.p, (size_t)nd * L, cudaMemcpyDeviceToHost, ws.stream));
+// Queues the copy of a chunk's dense rows (rows r0 .. r0 + nr - 1) into the pinned result, on the slot's stream.
+static int queue_dense_copy(b2t_result* r, const Workspace& ws, uint32_t r0, uint32_t nr, const DenseReq& dq) {
+  const size_t L = dq.L();
+  if (nr && L) {
+    CU(cudaMemcpyAsync(r->h_dense_ids.as<uint32_t>() + (size_t)r0 * L, ws.dense_ids.p, (size_t)nr * L * 4, cudaMemcpyDeviceToHost, ws.stream));
+    if (dq.want_mask) CU(cudaMemcpyAsync(r->h_dense_mask.as<uint8_t>() + (size_t)r0 * L, ws.dense_mask.p, (size_t)nr * L, cudaMemcpyDeviceToHost, ws.stream));
+    if (dq.pairs()) CU(cudaMemcpyAsync(r->h_type_ids.as<uint8_t>() + (size_t)r0 * L, ws.dense_type.p, (size_t)nr * L, cudaMemcpyDeviceToHost, ws.stream));
   }
-  if (nd) CU(cudaMemcpyAsync(r->h_row_len.as<uint32_t>() + d0, ws.dense_len.p, (size_t)nd * 4, cudaMemcpyDeviceToHost, ws.stream));
+  if (nr) CU(cudaMemcpyAsync(r->h_row_len.as<uint32_t>() + r0, ws.dense_len.p, (size_t)nr * 4, cudaMemcpyDeviceToHost, ws.stream));
   return B2T_OK;
 }
 
@@ -988,13 +1082,16 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
   if (dq && dq->batch_longest && total_bytes + n_docs >= (1ull << 31))
     return fail(B2T_ERR_UNSUPPORTED, "dense output padded to the longest row needs the batch in one device pass (< 2^31 bytes); pad to a fixed length instead");
   const uint64_t chunk_bytes = (dq && dq->batch_longest) ? (1ull << 31) : (uint64_t)e->chunk_bytes;
+  // chunks hold whole rows: per = documents per row (a pair's two documents stay in one chunk)
+  const uint32_t per = dq ? dq->docs_per_row : 1u, n_rows = n_docs / per;
   {
     uint32_t d = 0;
     while (d < n_docs) {
       uint64_t limit = doc_off[d] + chunk_bytes;
       uint32_t d1 = (uint32_t)(std::upper_bound(doc_off + d + 1, doc_off + n_docs + 1, limit) - doc_off) - 1;
-      if (d1 <= d) d1 = d + 1;  // a single document larger than the chunk size
-      if (doc_off[d1] - doc_off[d] >= (1ull << 31)) return fail(B2T_ERR_TOO_LARGE, "document %u is larger than 2 GiB", d);
+      d1 = d + (d1 - d) / per * per;
+      if (d1 <= d) d1 = d + per;  // a single row larger than the chunk size
+      if (doc_off[d1] - doc_off[d] >= (1ull << 31)) return fail(B2T_ERR_TOO_LARGE, per == 1 ? "document %u is larger than 2 GiB" : "pair %u is larger than 2 GiB", d / per);
       chunks.push_back({d, d1, doc_off[d], doc_off[d1], 0});
       max_chunk = std::max(max_chunk, doc_off[d1] - doc_off[d]);
       d = d1;
@@ -1002,7 +1099,7 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     if (chunks.empty()) chunks.push_back({0, 0, 0, 0, 0});
   }
   b2t_result* r = pool_get(e);
-  r->eng = e; r->on_device = 0; r->n_docs = n_docs; r->n_tokens = 0;
+  r->eng = e; r->on_device = 0; r->n_docs = dq ? n_rows : n_docs; r->n_tokens = 0;
   int rc;
   const bool want_off = (flags & B2T_WANT_OFFSETS) != 0, want_wid = (flags & B2T_WANT_WORD_IDS) != 0;
   // initial capacity guess: 0.30 tokens per byte, grown on demand (pinned pool => steady state allocates nothing)
@@ -1015,16 +1112,16 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     if (want_wid && (rc2 = r->h_word_ids.ensure(need_tok * 4, true))) return rc2;
     return B2T_OK;
   };
-  r->dense_len = 0; r->dense_ids = nullptr; r->dense_mask = nullptr; r->row_len = nullptr;
+  r->dense_len = 0; r->dense_ids = nullptr; r->dense_mask = nullptr; r->row_len = nullptr; r->type_ids = nullptr;
   auto dense_host = [&](uint32_t L) -> int {   // pinned rows of the whole batch
     int rc2;
-    const size_t cells = (size_t)n_docs * L;
-    if ((rc2 = r->h_dense_ids.ensure(cells * 4 + 16, false)) || (rc2 = r->h_row_len.ensure((size_t)n_docs * 4 + 16, false)) ||
-        (dq->want_mask && (rc2 = r->h_dense_mask.ensure(cells + 16, false))))
+    const size_t cells = (size_t)n_rows * L;
+    if ((rc2 = r->h_dense_ids.ensure(cells * 4 + 16, false)) || (rc2 = r->h_row_len.ensure((size_t)n_rows * 4 + 16, false)) ||
+        (dq->want_mask && (rc2 = r->h_dense_mask.ensure(cells + 16, false))) || (dq->pairs() && (rc2 = r->h_type_ids.ensure(cells + 16, false))))
       return rc2;
     return B2T_OK;
   };
-  if (dq) { if (!dq->batch_longest && (rc = dense_host(dq->S.L))) { pool_put(e, r); return rc; } }
+  if (dq) { if (!dq->batch_longest && (rc = dense_host(dq->L()))) { pool_put(e, r); return rc; } }
   else if ((rc = grow(cap_tok))) { pool_put(e, r); return rc; }
 
   uint64_t tok_base = 0;
@@ -1042,15 +1139,15 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     const uint64_t nt = ws.h_ctl.as<ctl_block>()->total;
     c.tok_base = tok_base;
     if (dq) {
-      const uint32_t nd = c.d1 - c.d0, max_row = ws.h_ctl.as<ctl_block>()->max_row;
+      const uint32_t nr = (c.d1 - c.d0) / per, max_row = ws.h_ctl.as<ctl_block>()->max_row;
       if (dq->batch_longest) {   // one chunk: L is known now
-        dq->S.L = dense_round(max_row, dq->multiple);
-        if ((rc2 = dense_host(dq->S.L)) || (rc2 = launch_dense(e, ws, nd, *dq, ws.stream))) return rc2;
-      } else if (max_row > dq->S.L) {
-        return fail(B2T_ERR_INVALID, "a row of %u tokens does not fit the dense length %u: enable truncation (the reference returns a longer row here)", max_row, dq->S.L);
+        dq->L() = dense_round(max_row, dq->multiple);
+        if ((rc2 = dense_host(dq->L())) || (rc2 = launch_dense(e, ws, nr, *dq, ws.stream))) return rc2;
+      } else if (max_row > dq->L()) {
+        return fail(B2T_ERR_INVALID, "a row of %u tokens does not fit the dense length %u: enable truncation (the reference returns a longer row here)", max_row, dq->L());
       }
       // (a fixed length: the rows were queued for the copy right behind the kernels, see issue(); a rerun has replaced them)
-      if ((dq->batch_longest || reran) && (rc2 = queue_dense_copy(r, ws, c.d0, nd, *dq))) return rc2;
+      if ((dq->batch_longest || reran) && (rc2 = queue_dense_copy(r, ws, c.d0 / per, nr, *dq))) return rc2;
       tok_base += nt;
       return B2T_OK;
     }
@@ -1092,7 +1189,7 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     if ((rc2 = run_device_pipeline(e, ws, ws.stream))) return rc2;
     // dense rows of a fixed length: their place in the result does not depend on anything the host has to read first, so
     // the copy back is queued right behind the kernels (the CSR modes need the chunk's token count for that)
-    if (dq && !dq->batch_longest && (rc2 = queue_dense_copy(r, ws, c.d0, nd, *dq))) return rc2;
+    if (dq && !dq->batch_longest && (rc2 = queue_dense_copy(r, ws, c.d0 / per, nd / per, *dq))) return rc2;
     CU(cudaEventRecord(ws.done, ws.stream));
     return B2T_OK;
   };
@@ -1108,11 +1205,12 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
   if (rc) { pool_put(e, r); return rc; }
 
   if (dq) {
-    if (n_docs == 0 && dq->batch_longest) dq->S.L = 0;
+    if (n_docs == 0 && dq->batch_longest) dq->L() = 0;
     r->n_tokens = tok_base; r->ids = nullptr; r->offsets = nullptr; r->word_ids = nullptr; r->row_ptr = nullptr;
-    r->dense_len = dq->S.L;
+    r->dense_len = dq->L();
     r->dense_ids = r->h_dense_ids.as<uint32_t>(); r->row_len = r->h_row_len.as<uint32_t>();
     r->dense_mask = dq->want_mask ? r->h_dense_mask.as<uint8_t>() : nullptr;
+    r->type_ids = dq->pairs() ? r->h_type_ids.as<uint8_t>() : nullptr;
   } else {
     // chunk-relative row_ptr -> batch-relative (host fix-up: one addition per document)
     uint64_t* rp = r->h_row_ptr.as<uint64_t>();
@@ -1133,9 +1231,9 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
 
 // The host-buffer entry points: argument checks (and in dense mode the spec, read into *dq), then `run(slot set)` on a slot
 // set of the call's own -- and, while per-kernel profiling is on, on the whole engine (the event records are one per engine).
-template <class Run>
+template <class Spec, class Run>
 static int host_call(const char* fn, b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, b2t_result** out,
-                     const b2t_dense_spec* spec, DenseReq* dq, Run&& run) {
+                     const Spec* spec, DenseReq* dq, Run&& run) {
   if (!e || !out || !doc_off || (!bytes && doc_off[n_docs])) return fail(B2T_ERR_INVALID, "%s: null argument", fn);
   int rc;
   if (dq && (rc = make_dense_req(spec, dq))) return rc;
@@ -1151,7 +1249,7 @@ static int host_call(const char* fn, b2t_engine* e, const uint8_t* bytes, const 
 
 extern "C" int b2t_encode_batch(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, uint32_t flags,
                                 b2t_result** out) {
-  return host_call("b2t_encode_batch", e, bytes, doc_off, n_docs, out, nullptr, nullptr,
+  return host_call("b2t_encode_batch", e, bytes, doc_off, n_docs, out, NO_SPEC, nullptr,
                    [&](b2t_engine::SlotSet& ss) { return host_encode(e, ss, bytes, doc_off, n_docs, flags, out); });
 }
 
@@ -1159,6 +1257,17 @@ extern "C" int b2t_encode_batch_dense(b2t_engine* e, const uint8_t* bytes, const
                                       b2t_result** out) {
   DenseReq dq;
   return host_call("b2t_encode_batch_dense", e, bytes, doc_off, n_docs, out, spec, &dq,
+                   [&](b2t_engine::SlotSet& ss) { return host_encode(e, ss, bytes, doc_off, n_docs, 0u, out, &dq); });
+}
+
+// Replaces TokenizerImpl::post_process for a batch of pairs (tokenizer/mod.rs:1265-1317), see include/b2t.h
+extern "C" int b2t_encode_pairs_dense(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_pairs, const b2t_pair_dense_spec* spec,
+                                      b2t_result** out) {
+  DenseReq dq;
+  uint32_t n_docs = 0;
+  int rc = pair_docs("b2t_encode_pairs_dense", n_pairs, &n_docs);
+  if (rc) return rc;
+  return host_call("b2t_encode_pairs_dense", e, bytes, doc_off, n_docs, out, spec, &dq,
                    [&](b2t_engine::SlotSet& ss) { return host_encode(e, ss, bytes, doc_off, n_docs, 0u, out, &dq); });
 }
 
@@ -1216,7 +1325,7 @@ static int pre_tokenize(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* b
 }
 
 extern "C" int b2t_pre_tokenize_batch(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, b2t_result** out) {
-  return host_call("b2t_pre_tokenize_batch", e, bytes, doc_off, n_docs, out, nullptr, nullptr,
+  return host_call("b2t_pre_tokenize_batch", e, bytes, doc_off, n_docs, out, NO_SPEC, nullptr,
                    [&](b2t_engine::SlotSet& ss) { return pre_tokenize(e, ss, bytes, doc_off, n_docs, out); });
 }
 
@@ -1232,6 +1341,7 @@ extern "C" uint32_t b2t_result_dense_length(const b2t_result* r) { return r ? r-
 extern "C" const uint32_t* b2t_result_dense_ids(const b2t_result* r) { return r ? r->dense_ids : nullptr; }
 extern "C" const uint8_t* b2t_result_attention_mask(const b2t_result* r) { return r ? r->dense_mask : nullptr; }
 extern "C" const uint32_t* b2t_result_row_lengths(const b2t_result* r) { return r ? r->row_len : nullptr; }
+extern "C" const uint8_t* b2t_result_type_ids(const b2t_result* r) { return r ? r->type_ids : nullptr; }
 extern "C" void b2t_result_free(b2t_result* r) {
   if (!r) return;
   if (r->on_device || !r->eng) { delete r; return; }

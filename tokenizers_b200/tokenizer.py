@@ -812,16 +812,13 @@ class Tokenizer:
         out._owner = be._owner   # the views die with the BatchEncoding
         return out
 
-    # ---- dense mode: template + truncation + padding on the device (include/b2t.h b2t_encode_batch_dense)
-    def dense_spec(self, add_special_tokens=True, want_mask=True):
-        """The tokenizer's truncation / padding / single-sequence template as a b2t_dense_spec (+ the arrays it points to)."""
-        tp, tr, pd = self._template, self._truncation, self._padding
+    # ---- dense mode: template + truncation + padding on the device (include/b2t.h b2t_encode_batch_dense, b2t_encode_pairs_dense)
+    def _dense_fields(self, sp, want_mask):
+        """the padding / truncation fields b2t_dense_spec and b2t_pair_dense_spec share, filled into sp"""
+        tr, pd = self._truncation, self._padding
         if pd is None:
             raise UnsupportedConfig("dense output needs padding enabled (enable_padding): rows must share one length")
-        pre = [t for t, _ in tp["pre"]] if (tp is not None and add_special_tokens) else []
-        post = [t for t, _ in tp["post"]] if (tp is not None and add_special_tokens) else []
-        sp = _lib.DenseSpec()
-        sp.struct_size = ctypes.sizeof(_lib.DenseSpec)
+        sp.struct_size = ctypes.sizeof(type(sp))
         sp.length = 0 if pd["length"] is None else int(pd["length"])
         sp.pad_to_multiple_of = int(pd["pad_to_multiple_of"] or 0)
         sp.max_length = 0 if tr is None else int(tr["max_length"])
@@ -830,11 +827,57 @@ class Tokenizer:
         sp.pad_id = pd["pad_id"]
         sp.truncate_left = int(tr is not None and tr["direction"] == "left")
         sp.pad_left = int(pd["direction"] == "left")
+        sp.want_mask = int(want_mask)
+        return sp
+
+    def dense_spec(self, add_special_tokens=True, want_mask=True):
+        """The tokenizer's truncation / padding / single-sequence template as a b2t_dense_spec (+ the arrays it points to)."""
+        tp = self._template
+        pre = [t for t, _ in tp["pre"]] if (tp is not None and add_special_tokens) else []
+        post = [t for t, _ in tp["post"]] if (tp is not None and add_special_tokens) else []
+        sp = self._dense_fields(_lib.DenseSpec(), want_mask)
         keep = (np.asarray(pre, dtype=np.uint32), np.asarray(post, dtype=np.uint32))
         sp.n_pre, sp.n_post = len(pre), len(post)
         sp.pre_ids, sp.post_ids = (keep[0].ctypes.data if pre else None), (keep[1].ctypes.data if post else None)
-        sp.want_mask = int(want_mask)
         return sp, keep
+
+    def pair_dense_spec(self, add_special_tokens=True, want_mask=True):
+        """The tokenizer's truncation / padding / pair template as a b2t_pair_dense_spec (+ the arrays it points to).  The
+        pieces come from the template's pair form (default_process without a post-processor: A type 0, B type 1); without
+        special tokens the two sequence pieces stay, in their order and with their type ids (processors/template.rs:554-560)."""
+        tp, tr, pd = self._template, self._truncation, self._padding
+        pieces = [("seq", 0, 0), ("seq", 1, 1)] if tp is None else tp["pair"]
+        if pieces is None:
+            raise ValueError("the post-processor has no template for pairs of sequences")
+        sp = self._dense_fields(_lib.PairDenseSpec(), want_mask)
+        pieces = [p for p in pieces if p[0] == "seq" or add_special_tokens]
+        if tr is not None:
+            if tr["stride"]:
+                raise UnsupportedConfig("stride only shapes overflowing parts, which have no dense form")
+            # the engine truncates the pair to max_length less the special tokens it is given: the budget of the reference
+            sp.max_length = truncation_budget(tr, tp, True, add_special_tokens) + sum(1 for p in pieces if p[0] == "special")
+            sp.strategy = {"longest_first": _lib.TRUNC_LONGEST_FIRST, "only_first": _lib.TRUNC_ONLY_FIRST, "only_second": _lib.TRUNC_ONLY_SECOND}[tr["strategy"]]
+        sp.pad_type_id = pd["pad_type_id"]
+        keep = (np.asarray([v if k == "special" else (_lib.PIECE_A if v == 0 else _lib.PIECE_B) for k, v, _ in pieces], dtype=np.uint32),
+                np.asarray([t for _, _, t in pieces], dtype=np.uint32))
+        sp.n_pieces, sp.piece_ids, sp.piece_types = len(pieces), keep[0].ctypes.data, keep[1].ctypes.data
+        return sp, keep
+
+    def _dense_call(self, entry, data, doc_off, n_rows, sp, want_mask, type_ids):
+        """b2t_encode_batch_dense / b2t_encode_pairs_dense -> (ids [n, L], mask [n, L] | None, lengths [n], type ids [n, L] | None)"""
+        if self._added is not None and not self._dev_added and added.split_batch(self._added, data, doc_off)[2]:
+            raise UnsupportedConfig("the batch contains added tokens and this configuration extracts them on the host: use encode_batch")
+        L = _lib.lib()
+        res = ctypes.c_void_p()
+        _lib.check(getattr(L, entry)(self._h, data.ctypes.data if data.size else None, doc_off.ctypes.data, n_rows, ctypes.byref(sp), ctypes.byref(res)))
+
+        def views(L, res):
+            W = L.b2t_result_dense_length(res)
+            return (_view(L.b2t_result_dense_ids(res), n_rows * W, np.uint32).reshape(n_rows, W),
+                    _view(L.b2t_result_attention_mask(res), n_rows * W, np.uint8).reshape(n_rows, W) if want_mask else None,
+                    _view(L.b2t_result_row_lengths(res), n_rows, np.uint32),
+                    _view(L.b2t_result_type_ids(res), n_rows * W, np.uint8).reshape(n_rows, W) if type_ids else None)
+        return _read_result(self, res, views)[0]
 
     def encode_batch_dense(self, data, doc_off=None, add_special_tokens=True, want_mask=True):
         """Batch of single sequences -> {"input_ids": uint32[n, L], "attention_mask": uint8[n, L] | None, "lengths": uint32[n]}
@@ -844,22 +887,38 @@ class Tokenizer:
             data, doc_off = _pack(data, np.uint64)
         data = np.ascontiguousarray(data, dtype=np.uint8)
         doc_off = np.ascontiguousarray(doc_off, dtype=np.uint64)
-        if self._added is not None and not self._dev_added and added.split_batch(self._added, data, doc_off)[2]:
-            raise UnsupportedConfig("the batch contains added tokens and this configuration extracts them on the host: use encode_batch")
         sp, keep = self.dense_spec(add_special_tokens, want_mask)
-        n = len(doc_off) - 1
-        L = _lib.lib()
-        res = ctypes.c_void_p()
-        _lib.check(L.b2t_encode_batch_dense(self._h, data.ctypes.data if data.size else None, doc_off.ctypes.data, n, ctypes.byref(sp), ctypes.byref(res)))
-        del keep
-
-        def views(L, res):
-            W = L.b2t_result_dense_length(res)
-            return (_view(L.b2t_result_dense_ids(res), n * W, np.uint32).reshape(n, W),
-                    _view(L.b2t_result_attention_mask(res), n * W, np.uint8).reshape(n, W) if want_mask else None,
-                    _view(L.b2t_result_row_lengths(res), n, np.uint32))
-        (ids, mask, lens), _ = _read_result(self, res, views)
+        ids, mask, lens, _ = self._dense_call("b2t_encode_batch_dense", data, doc_off, len(doc_off) - 1, sp, want_mask, False)
         return {"input_ids": ids, "attention_mask": mask, "lengths": lens}
+
+    def encode_pairs_dense(self, pairs, doc_off=None, add_special_tokens=True, want_mask=True):
+        """Batch of pairs of sequences -> {"input_ids": uint32[n, L], "token_type_ids": uint8[n, L], "attention_mask": uint8[n, L]
+        | None, "lengths": uint32[n]} with the tokenizer's pair truncation, pair template and padding applied on the device
+        (what `encode_batch` on pairs + stacking the Encodings' ids / type_ids / attention_mask gives in the reference).
+        `pairs` is a list of (str, str), or packed (np.uint8[N], np.uint64[2n+1]): document 2p is the first sequence of
+        pair p, 2p + 1 the second.  A pair that cannot be truncated raises ValueError as the reference does; stride
+        (overflowing parts) has no dense form."""
+        if doc_off is None:
+            seqs = []
+            for x in pairs:
+                if not (isinstance(x, (tuple, list)) and len(x) == 2 and all(isinstance(t, str) for t in x)):
+                    raise TypeError("encode_pairs_dense expects pairs (str, str)")
+                seqs.extend(x)
+            pairs, doc_off = _pack(seqs, np.uint64)
+        data = np.ascontiguousarray(pairs, dtype=np.uint8)
+        doc_off = np.ascontiguousarray(doc_off, dtype=np.uint64)
+        if len(doc_off) % 2 != 1:
+            raise ValueError(f"a batch of n pairs has 2n + 1 document offsets, not {len(doc_off)}")
+        sp, keep = self.pair_dense_spec(add_special_tokens, want_mask)
+        try:
+            ids, mask, lens, types = self._dense_call("b2t_encode_pairs_dense", data, doc_off, (len(doc_off) - 1) // 2, sp, want_mask, True)
+        except B2TError as ex:
+            if ex.code == _lib.B2T_ERR_TRUNCATION:   # TruncationError::SequenceTooShort, with the reference's message
+                raise ValueError(str(ex)) from None
+            if ex.code == _lib.B2T_ERR_UNSUPPORTED:
+                raise UnsupportedConfig(str(ex)) from None
+            raise
+        return {"input_ids": ids, "token_type_ids": types, "attention_mask": mask, "lengths": lens}
 
     def _trim_tables(self):
         """per token id: leading / trailing 'G-dot' characters (the byte-level image of U+0020) of its vocabulary string"""
