@@ -30,7 +30,9 @@ typedef enum {
   B2T_ERR_CUDA = 3,        /* CUDA runtime error, message has the details */
   B2T_ERR_VOCAB = 4,       /* merge token out of vocabulary / missing [UNK] (models/bpe/mod.rs:12-36, wordpiece/mod.rs:17-22) */
   B2T_ERR_TOO_LARGE = 5,   /* batch exceeds the per-call device limits */
-  B2T_ERR_TRUNCATION = 6   /* TruncationError::SequenceTooShort (utils/truncation.rs:155): a pair cannot be cut to max_length */
+  B2T_ERR_TRUNCATION = 6   /* TruncationError::SequenceTooShort (utils/truncation.rs:155): a pair cannot be cut to max_length;
+                              or, with overflowing parts, a sequence that has to be cut to a max_len no larger than the
+                              stride (the reference panics there: tokenizer/encoding.rs:318) */
 } b2t_status;
 
 /* models::ModelWrapper variants on the path (models/mod.rs:60-68) */
@@ -145,7 +147,15 @@ int b2t_encode_batch_device_finish(b2t_engine* e, uint32_t* d_ids, uint32_t* d_o
  * `pre $A post` (processors/template.rs:646-, BertProcessing / RobertaProcessing single form) and padding
  * (utils/padding.rs:50-81), as TokenizerImpl::post_process orders them (tokenizer/mod.rs:1265-1317) -- done on the device:
  * the result is a dense [n_docs, L] tensor of ids (+ attention mask + row lengths) instead of the token CSR, which never
- * leaves the device.  Overflowing parts (stride) are not part of a dense batch; offsets are not produced. */
+ * leaves the device.  With B2T_DENSE_OVERFLOW the overflowing parts (stride) of a truncated sequence become rows of their own,
+ * and with B2T_DENSE_OFFSETS the character offsets of every position come back too (see below). */
+enum {
+  B2T_DENSE_OVERFLOW = 1u,  /* return_overflowing_tokens: every part Encoding::truncate makes (tokenizer/encoding.rs:307-388) is a
+                               row -- an input's kept row first, then its overflowing rows (`[e] + e.overflowing`), each with the
+                               template around it; b2t_result_row_sample maps each row to its input */
+  B2T_DENSE_OFFSETS = 2u    /* return_offsets_mapping: [rows, L] (start, end) char offsets relative to the row's sequence
+                               (growing_offsets = false), (0, 0) for special tokens and padding */
+};
 typedef struct {
   uint32_t struct_size;        /* sizeof(b2t_dense_spec) */
   uint32_t length;             /* PaddingStrategy::Fixed(length); 0 = BatchLongest (needs the batch in one device pass: < 2^31 bytes) */
@@ -158,28 +168,43 @@ typedef struct {
   const uint32_t* pre_ids;
   const uint32_t* post_ids;
   uint32_t want_mask;          /* also return the attention mask (u8 per position); row lengths always come back */
+  /* appended fields: a struct_size that ends before them (the size of the struct without them) reads them as 0 */
+  uint32_t stride;             /* TruncationParams.stride: tokens consecutive parts share (B2T_DENSE_OVERFLOW only) */
+  uint32_t dense_flags;        /* B2T_DENSE_* */
 } b2t_dense_spec;
 
 /* HOST buffers in (as b2t_encode_batch), pinned host rows out.  A row that does not fit L (Fixed length without a
- * sufficient truncation; the reference returns a longer row there) fails the batch with B2T_ERR_INVALID. */
+ * sufficient truncation; the reference returns a longer row there) fails the batch with B2T_ERR_INVALID.  With
+ * B2T_DENSE_OVERFLOW, L is still the longest KEPT row under BatchLongest (pad_encodings looks at the top-level encodings
+ * only), and an overflowing row longer than L fails the batch the same way (the reference returns it unpadded and longer:
+ * a whole sequence overflows when it is cut to 0 tokens). */
 int b2t_encode_batch_dense(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs,
                            const b2t_dense_spec* spec, b2t_result** out);
 /* Device buffers in (as b2t_encode_batch_device), device rows out (owned by the engine until the next call). */
 int b2t_encode_batch_dense_device(b2t_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off,
                                   uint32_t n_docs, const b2t_dense_spec* spec, void* stream, b2t_result** out);
-/* Dense results: row d = ids[d * L .. (d + 1) * L); row_lengths[d] = tokens of row d that are not padding. */
+/* Dense results: R rows (R = b2t_result_n_docs without B2T_DENSE_OVERFLOW); row d = ids[d * L .. (d + 1) * L);
+ * row_lengths[d] = tokens of row d that are not padding.  b2t_result_n_docs stays the number of inputs. */
 uint32_t b2t_result_dense_length(const b2t_result* r);        /* L */
-const uint32_t* b2t_result_dense_ids(const b2t_result* r);    /* n_docs * L */
-const uint8_t* b2t_result_attention_mask(const b2t_result* r); /* n_docs * L, or NULL */
-const uint32_t* b2t_result_row_lengths(const b2t_result* r);  /* n_docs */
+uint32_t b2t_result_dense_rows(const b2t_result* r);          /* R (0 for a result that is not dense); R < 2^31, else the call
+                                                                 fails with B2T_ERR_TOO_LARGE */
+const uint32_t* b2t_result_dense_ids(const b2t_result* r);    /* R * L */
+const uint8_t* b2t_result_attention_mask(const b2t_result* r); /* R * L, or NULL */
+const uint32_t* b2t_result_row_lengths(const b2t_result* r);  /* R */
+const uint32_t* b2t_result_row_sample(const b2t_result* r);   /* R: the input of each row (overflow_to_sample_mapping), or NULL
+                                                                 without B2T_DENSE_OVERFLOW */
+const uint32_t* b2t_result_dense_offsets(const b2t_result* r); /* R * L * 2 (start, end), or NULL without B2T_DENSE_OFFSETS */
 
 /* Dense mode for PAIRS of sequences (EncodeInput::Dual): what the reference runs after the path for a batch of pairs --
  * truncate_encodings with a pair (utils/truncation.rs:70-162, kept parts only), the pair template (processors/template.rs:
  * 544-643 apply_template; BertProcessing / RobertaProcessing pair forms; default_process without a post-processor) and
  * padding (utils/padding.rs:50-81), as TokenizerImpl::post_process orders them (tokenizer/mod.rs:1265-1317) -- done on the
  * device.  The batch is 2 n_pairs documents: document 2p is the first sequence of pair p, 2p + 1 the second.  The result
- * is n_pairs dense rows of ids, type ids (+ attention mask + row lengths); b2t_result_n_docs is n_pairs.  Overflowing parts
- * (stride) are not part of a dense batch. */
+ * is n_pairs dense rows of ids, type ids (+ attention mask + row lengths); b2t_result_n_docs is n_pairs.  With
+ * B2T_DENSE_OVERFLOW each sequence is cut with the max_len truncate_encodings gives it, and a pair whose sequences have
+ * 1 + o_x and 1 + o_y parts (X / Y = first / second sequence in template order) gives (1 + o_x)(1 + o_y) rows in
+ * Encoding::merge_with's order (tokenizer/encoding.rs:408-463): (0, 0); (i, 0), (i, 1) .. (i, o_y) for i = 1 .. o_x; then
+ * (0, 1) .. (0, o_y).  A kept part takes its piece's type id, an overflowing part overflow_type_a / _b. */
 enum { B2T_TRUNC_LONGEST_FIRST = 0, B2T_TRUNC_ONLY_FIRST = 1, B2T_TRUNC_ONLY_SECOND = 2 };  /* TruncationStrategy */
 /* the sequence pieces of a template's piece list (token ids are < 2^20, so these never collide with one) */
 enum { B2T_PIECE_A = 0x80000000u, B2T_PIECE_B = 0x80000001u };
@@ -201,6 +226,11 @@ typedef struct {
   const uint32_t* piece_ids;
   const uint32_t* piece_types;
   uint32_t want_mask;          /* also return the attention mask (u8 per position); type ids and row lengths always come back */
+  /* appended fields: a struct_size that ends before them (the size of the struct without them) reads them as 0 */
+  uint32_t stride;             /* TruncationParams.stride (B2T_DENSE_OVERFLOW only) */
+  uint32_t dense_flags;        /* B2T_DENSE_* */
+  uint32_t overflow_type_a;    /* type id of the overflowing parts of A / B (<= 255): the type id they had before the template, */
+  uint32_t overflow_type_b;    /* 0 / 1 -- 0 / 0 under RobertaProcessing with special tokens (processors/roberta.rs) */
 } b2t_pair_dense_spec;
 
 /* HOST buffers in (doc_off holds 2 n_pairs + 1 offsets), pinned host rows out.  A pair that cannot be truncated fails the

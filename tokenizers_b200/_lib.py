@@ -12,6 +12,7 @@ WANT_OFFSETS, WANT_WORD_IDS, OFFSETS_BYTES, NO_ADDED_TOKENS, FLAG_ADDED_IDS = 1,
 ADDED_SINGLE_WORD, ADDED_LSTRIP, ADDED_RSTRIP, ADDED_NORMALIZED = 1, 2, 4, 8
 TRUNC_LONGEST_FIRST, TRUNC_ONLY_FIRST, TRUNC_ONLY_SECOND = 0, 1, 2
 PIECE_A, PIECE_B = 0x80000000, 0x80000001
+DENSE_OVERFLOW, DENSE_OFFSETS = 1, 2
 
 # every symbol include/b2t.h declares
 SYMBOLS = ["b2t_engine_create", "b2t_engine_destroy", "b2t_engine_set_added_tokens", "b2t_encode_batch", "b2t_encode_batch_device", "b2t_encode_batch_device_begin",
@@ -19,6 +20,7 @@ SYMBOLS = ["b2t_engine_create", "b2t_engine_destroy", "b2t_engine_set_added_toke
            "b2t_encode_batch_dense", "b2t_encode_batch_dense_device", "b2t_result_dense_length", "b2t_result_dense_ids",
            "b2t_result_attention_mask", "b2t_result_row_lengths",
            "b2t_encode_pairs_dense", "b2t_encode_pairs_dense_device", "b2t_result_type_ids",
+           "b2t_result_dense_rows", "b2t_result_row_sample", "b2t_result_dense_offsets",
            "b2t_result_n_tokens", "b2t_result_n_docs", "b2t_result_on_device", "b2t_result_ids", "b2t_result_offsets",
            "b2t_result_word_ids", "b2t_result_row_ptr", "b2t_result_free", "b2t_host_alloc", "b2t_host_free",
            "b2t_engine_set_profiling", "b2t_engine_last_kernels", "b2t_unicode_class_table", "b2t_bert_normalizer_images", "b2t_last_error", "b2t_version"]
@@ -38,7 +40,7 @@ class DenseSpec(ctypes.Structure):
     _fields_ = [("struct_size", ctypes.c_uint32), ("length", ctypes.c_uint32), ("pad_to_multiple_of", ctypes.c_uint32),
                 ("max_length", ctypes.c_uint32), ("pad_id", ctypes.c_uint32), ("truncate_left", ctypes.c_int32), ("pad_left", ctypes.c_int32),
                 ("n_pre", ctypes.c_uint32), ("n_post", ctypes.c_uint32), ("pre_ids", ctypes.c_void_p), ("post_ids", ctypes.c_void_p),
-                ("want_mask", ctypes.c_uint32)]
+                ("want_mask", ctypes.c_uint32), ("stride", ctypes.c_uint32), ("dense_flags", ctypes.c_uint32)]
 
 
 class PairDenseSpec(ctypes.Structure):
@@ -46,7 +48,11 @@ class PairDenseSpec(ctypes.Structure):
                 ("max_length", ctypes.c_uint32), ("strategy", ctypes.c_int32), ("truncate_left", ctypes.c_int32),
                 ("pad_id", ctypes.c_uint32), ("pad_type_id", ctypes.c_uint32), ("pad_left", ctypes.c_int32),
                 ("n_pieces", ctypes.c_uint32), ("piece_ids", ctypes.c_void_p), ("piece_types", ctypes.c_void_p),
-                ("want_mask", ctypes.c_uint32)]
+                ("want_mask", ctypes.c_uint32), ("stride", ctypes.c_uint32), ("dense_flags", ctypes.c_uint32),
+                ("overflow_type_a", ctypes.c_uint32), ("overflow_type_b", ctypes.c_uint32)]
+
+# the specs' size before stride and dense_flags were appended (accepted by the engine: those fields read as 0)
+DENSE_SPEC_V1_SIZE = PAIR_DENSE_SPEC_V1_SIZE = 64
 
 
 class B2TError(RuntimeError):
@@ -81,7 +87,9 @@ def lib():
     L.b2t_result_dense_length.argtypes = [vp]; L.b2t_result_dense_length.restype = u32
     L.b2t_encode_pairs_dense.argtypes = [vp, vp, vp, u32, ctypes.POINTER(PairDenseSpec), ctypes.POINTER(vp)]
     L.b2t_encode_pairs_dense_device.argtypes = [vp, vp, u64, vp, u32, ctypes.POINTER(PairDenseSpec), vp, ctypes.POINTER(vp)]
-    for f in ("b2t_result_dense_ids", "b2t_result_attention_mask", "b2t_result_row_lengths", "b2t_result_type_ids"):
+    L.b2t_result_dense_rows.argtypes = [vp]; L.b2t_result_dense_rows.restype = u32
+    for f in ("b2t_result_dense_ids", "b2t_result_attention_mask", "b2t_result_row_lengths", "b2t_result_type_ids", "b2t_result_row_sample",
+              "b2t_result_dense_offsets"):
         getattr(L, f).argtypes = [vp]; getattr(L, f).restype = vp
     L.b2t_result_n_tokens.argtypes = [vp]; L.b2t_result_n_tokens.restype = u64
     L.b2t_result_n_docs.argtypes = [vp]; L.b2t_result_n_docs.restype = u32

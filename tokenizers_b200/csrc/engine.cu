@@ -127,6 +127,9 @@ struct DenseReq {
   bool batch_longest = false;   // padding strategy BatchLongest: L = longest row of the batch (after pad_to_multiple_of)
   uint32_t multiple = 0;        // pad_to_multiple_of
   bool want_mask = false;
+  // overflowing parts (B2T_DENSE_OVERFLOW): rows per input are known after the count pass; offset rows (B2T_DENSE_OFFSETS)
+  bool overflow = false, offsets = false;
+  uint32_t stride = 0, type_oa = 0, type_ob = 0;
   bool pairs() const { return docs_per_row == 2; }
   uint32_t& L() { return pairs() ? P.L : S.L; }
   uint32_t L() const { return pairs() ? P.L : S.L; }
@@ -162,6 +165,7 @@ struct Workspace {
   unsigned long long pool_cap = 0;
   DevBuf wcache;                      // per-batch word cache (model_kernels.cuh)
   DevBuf dense_ids, dense_mask, dense_len, dense_type;  // dense [n_rows, L] rows (dense_kernels.cuh); type ids: pairs only
+  DevBuf dense_off, row_count, row_lexcl, row_bsum, row_base, row_sample;  // overflow rows: offset rows, the count pass and its scan
   // BertNormalizer pre-pass (norm_kernels.cuh): the normalized batch and what maps its tokens back to the original
   DevBuf nrm_doc_bits, nrm_pfd, nrm_page_out, nrm_page_chars, nrm_lexcl_o, nrm_bsum_o, nrm_lexcl_c, nrm_bsum_c, nrm_tot, nrm_bytes, nrm_src_char, nrm_doc_off, nrm_doc_char0;
   bool norm_active = false;
@@ -189,7 +193,9 @@ struct b2t_result {
   uint32_t dense_len = 0;
   const uint32_t* dense_ids = nullptr; const uint8_t* dense_mask = nullptr; const uint32_t* row_len = nullptr;
   const uint8_t* type_ids = nullptr;
-  PinBuf h_dense_ids, h_dense_mask, h_row_len, h_type_ids;
+  uint32_t n_rows = 0;   // dense rows R (n_docs without overflowing parts)
+  const uint32_t* row_sample = nullptr; const uint32_t* dense_off = nullptr;
+  PinBuf h_dense_ids, h_dense_mask, h_row_len, h_type_ids, h_row_sample, h_dense_off;
 };
 
 constexpr int NSLOT = 3;   // chunk workspaces of one host-path call: NSLOT - 1 chunks are in flight while the next is issued
@@ -346,6 +352,9 @@ struct ctl_block {  // lives in ws.ctl
   unsigned long long total;
   LongCtl lc;
   uint32_t added_used;   // entries of the added-token list pool handed out
+  uint32_t max_all;      // dense mode with overflowing parts: longest of all rows
+  unsigned long long rows;   // dense mode with overflowing parts: rows of the batch
+  uint32_t stride_m;     // ERR_STRIDE: the max_len the reference would panic on
   uint32_t pad;
 };
 
@@ -407,10 +416,33 @@ static uint32_t dense_round(uint32_t len, uint32_t multiple) {
   if (multiple > 0 && len % multiple) len += multiple - len % multiple;
   return len;
 }
+// A spec read at the caller's struct_size: the current size, or the size before the fields from `stride` on were appended
+// (those read as 0).  false = neither.
+template <class Spec>
+static bool read_spec(const Spec* sp, Spec* out) {
+  constexpr size_t head = offsetof(Spec, stride), head_size = (head + 7) & ~(size_t)7;   // the old sizeof, tail padding included
+  if (sp->struct_size != sizeof(Spec) && sp->struct_size != head_size) return false;
+  memset(out, 0, sizeof(Spec));
+  memcpy(out, sp, sp->struct_size == sizeof(Spec) ? sizeof(Spec) : head);
+  return true;
+}
+static_assert(offsetof(b2t_dense_spec, stride) == 60 && offsetof(b2t_pair_dense_spec, stride) == 60, "the specs' first layout was 64 bytes");
+
+static int dense_flags(uint32_t flags, uint32_t stride, DenseReq* dq) {
+  if (flags & ~(uint32_t)(B2T_DENSE_OVERFLOW | B2T_DENSE_OFFSETS)) return fail(B2T_ERR_INVALID, "unknown dense_flags 0x%x", flags);
+  dq->overflow = (flags & B2T_DENSE_OVERFLOW) != 0; dq->offsets = (flags & B2T_DENSE_OFFSETS) != 0;
+  dq->stride = dq->overflow ? stride : 0u;
+  return B2T_OK;
+}
+
 // b2t_dense_spec -> DenseReq, checked
-static int make_dense_req(const b2t_dense_spec* sp, DenseReq* dq) {
-  if (!sp) return fail(B2T_ERR_INVALID, "dense spec is null");
-  if (sp->struct_size != sizeof(b2t_dense_spec)) return fail(B2T_ERR_INVALID, "b2t_dense_spec: struct_size mismatch (%u != %zu)", sp->struct_size, sizeof(b2t_dense_spec));
+static int make_dense_req(const b2t_dense_spec* sp_in, DenseReq* dq) {
+  if (!sp_in) return fail(B2T_ERR_INVALID, "dense spec is null");
+  b2t_dense_spec spec;
+  if (!read_spec(sp_in, &spec)) return fail(B2T_ERR_INVALID, "b2t_dense_spec: struct_size mismatch (%u != %zu)", sp_in->struct_size, sizeof(b2t_dense_spec));
+  const b2t_dense_spec* sp = &spec;
+  int rc;
+  if ((rc = dense_flags(sp->dense_flags, sp->stride, dq))) return rc;
   if (sp->n_pre > (uint32_t)DENSE_MAX_SPECIAL || sp->n_post > (uint32_t)DENSE_MAX_SPECIAL)
     return fail(B2T_ERR_UNSUPPORTED, "templates with more than %d special tokens on one side are not supported", DENSE_MAX_SPECIAL);
   if ((sp->n_pre && !sp->pre_ids) || (sp->n_post && !sp->post_ids)) return fail(B2T_ERR_INVALID, "dense spec: null special-token list");
@@ -430,10 +462,17 @@ static int make_dense_req(const b2t_dense_spec* sp, DenseReq* dq) {
   return B2T_OK;
 }
 // b2t_pair_dense_spec -> DenseReq (pairs), checked: the piece list is split into pre X mid Y post
-static int make_dense_req(const b2t_pair_dense_spec* sp, DenseReq* dq) {
-  if (!sp) return fail(B2T_ERR_INVALID, "pair dense spec is null");
-  if (sp->struct_size != sizeof(b2t_pair_dense_spec))
-    return fail(B2T_ERR_INVALID, "b2t_pair_dense_spec: struct_size mismatch (%u != %zu)", sp->struct_size, sizeof(b2t_pair_dense_spec));
+static int make_dense_req(const b2t_pair_dense_spec* sp_in, DenseReq* dq) {
+  if (!sp_in) return fail(B2T_ERR_INVALID, "pair dense spec is null");
+  b2t_pair_dense_spec spec;
+  if (!read_spec(sp_in, &spec))
+    return fail(B2T_ERR_INVALID, "b2t_pair_dense_spec: struct_size mismatch (%u != %zu)", sp_in->struct_size, sizeof(b2t_pair_dense_spec));
+  const b2t_pair_dense_spec* sp = &spec;
+  int rc;
+  if ((rc = dense_flags(sp->dense_flags, sp->stride, dq))) return rc;
+  if (dq->overflow && (sp->overflow_type_a > 255 || sp->overflow_type_b > 255))
+    return fail(B2T_ERR_UNSUPPORTED, "overflow type ids %u / %u: type ids above 255 are not supported", sp->overflow_type_a, sp->overflow_type_b);
+  dq->type_oa = sp->overflow_type_a; dq->type_ob = sp->overflow_type_b;
   if (sp->n_pieces && (!sp->piece_ids || !sp->piece_types)) return fail(B2T_ERR_INVALID, "pair dense spec: null piece list");
   if (sp->strategy < B2T_TRUNC_LONGEST_FIRST || sp->strategy > B2T_TRUNC_ONLY_SECOND) return fail(B2T_ERR_INVALID, "unknown truncation strategy %d", sp->strategy);
   if (sp->pad_type_id > 255) return fail(B2T_ERR_UNSUPPORTED, "pad type id %u: type ids above 255 are not supported", sp->pad_type_id);
@@ -476,13 +515,58 @@ static int make_dense_req(const b2t_pair_dense_spec* sp, DenseReq* dq) {
   return B2T_OK;
 }
 
-// CSR of the workspace -> dense rows in ws.dense_* (asynchronous on st); n_rows = documents / docs_per_row
-static int launch_dense(b2t_engine* e, Workspace& ws, uint32_t n_rows, const DenseReq& dq, cudaStream_t st) {
+template <bool OVER, bool OFFS>
+static void launch_rows(Workspace& ws, uint32_t n_rows, const DenseReq& dq, const DenseOverflow& O, cudaStream_t st) {
+  const unsigned grid = (unsigned)(((uint64_t)n_rows * 32 + 255) / 256);
+  if (dq.pairs())
+    dense_pair_rows_kernel<OVER, OFFS><<<grid, 256, 0, st>>>(ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.P, ws.dense_ids.as<uint32_t>(),
+                                                             ws.dense_type.as<uint8_t>(), dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr,
+                                                             ws.dense_len.as<uint32_t>(), O);
+  else
+    dense_rows_kernel<OVER, OFFS><<<grid, 256, 0, st>>>(ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.S, ws.dense_ids.as<uint32_t>(),
+                                                        dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr, ws.dense_len.as<uint32_t>(), nullptr, O);
+}
+
+// CSR of the workspace -> dense rows in ws.dense_* (asynchronous on st).  n_inputs = documents / docs_per_row; n_rows =
+// n_inputs, or with overflowing parts the rows the count pass found (the host has read them), whose row_sample entries
+// are the inputs' indices + sample_base.
+static int launch_dense(b2t_engine* e, Workspace& ws, uint32_t n_inputs, uint32_t n_rows, const DenseReq& dq, cudaStream_t st, uint32_t sample_base = 0) {
   int rc;
   const size_t cells = (size_t)n_rows * dq.L();
   if ((rc = ws.dense_ids.ensure(cells * 4 + 16)) || (rc = ws.dense_len.ensure((size_t)n_rows * 4 + 16)) ||
       (dq.want_mask && (rc = ws.dense_mask.ensure(cells + 16))) || (dq.pairs() && (rc = ws.dense_type.ensure(cells + 16))))
     return rc;
+  if (dq.overflow) {
+    if ((rc = ws.row_base.ensure((size_t)n_inputs * 4 + 16)) || (rc = ws.row_sample.ensure((size_t)n_rows * 4 + 16)) ||
+        (dq.offsets && (rc = ws.dense_off.ensure(cells * 8 + 16))))
+      return rc;
+    if (n_inputs)
+      dense_row_sample_kernel<<<(unsigned)(((uint64_t)n_inputs * 32 + 255) / 256), 256, 0, st>>>(
+          ws.row_count.as<uint32_t>(), ws.row_lexcl.as<unsigned long long>(), ws.row_bsum.as<unsigned long long>(), TSCAN, n_inputs, sample_base,
+          ws.row_base.as<uint32_t>(), ws.row_sample.as<uint32_t>());
+    e->last_launches++;
+    rec(e, st, "dense_row_sample");   // (from the end of dense_count: includes the host's read of the row count)
+    const bool b_first = dq.pairs() && dq.P.b_first;
+    DenseOverflow O{ws.row_sample.as<uint32_t>(), ws.row_base.as<uint32_t>(), sample_base, dq.stride,
+                    b_first ? dq.type_ob : dq.type_oa, b_first ? dq.type_oa : dq.type_ob,
+                    dq.offsets ? ws.offsets.as<uint2>() : nullptr, dq.offsets ? ws.dense_off.as<uint2>() : nullptr};
+    if (n_rows && dq.L()) {
+      if (dq.offsets) launch_rows<true, true>(ws, n_rows, dq, O, st);
+      else launch_rows<true, false>(ws, n_rows, dq, O, st);
+    }
+    e->last_launches++;
+    rec(e, st, dq.pairs() ? "dense_pair_rows_overflow" : "dense_rows_overflow");
+    CU(cudaGetLastError());
+    return B2T_OK;
+  }
+  if (dq.offsets) {   // offset rows of the kept parts only: the <0, 1> instantiations
+    if ((rc = ws.dense_off.ensure(cells * 8 + 16))) return rc;
+    const DenseOverflow O{nullptr, nullptr, 0u, 0u, 0u, 0u, ws.offsets.as<uint2>(), ws.dense_off.as<uint2>()};
+    if (n_rows && dq.L()) launch_rows<false, true>(ws, n_rows, dq, O, st);
+    e->last_launches++;
+    CU(cudaGetLastError());
+    return B2T_OK;
+  }
   const unsigned grid = (unsigned)(((uint64_t)n_rows * 32 + 255) / 256);
   if (n_rows && dq.L() && dq.pairs())
     dense_pair_rows_kernel<<<grid, 256, 0, st>>>(ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.P, ws.dense_ids.as<uint32_t>(),
@@ -751,8 +835,27 @@ static int finish_tail(b2t_engine* e, Workspace& ws, cudaStream_t st) {
     else if (n_rows)
       row_len_max_kernel<<<(n_rows + 255) / 256, 256, 0, st>>>(ws.row_ptr.as<uint64_t>(), n_rows, dq->S.keep_max, dq->S.n_pre + dq->S.n_post, &ctl->max_row);
     e->last_launches++;
-    if (!dq->batch_longest && (rc = launch_dense(e, ws, n_rows, *dq, st))) return rc;
-    rec(e, st, dq->pairs() ? "dense_pair_rows" : "dense_rows");
+    if (dq->overflow) {
+      // the rows of every input and the longest of them; an exclusive scan of the counts gives each input's first row
+      // (the rows themselves follow once the host has read the total)
+      const uint32_t budget = dq->pairs() ? P.budget : dq->S.keep_max, n_special = dq->pairs() ? P.n_pre + P.n_mid + P.n_post : dq->S.n_pre + dq->S.n_post;
+      const int64_t n_blk = ((int64_t)n_rows + TSCAN - 1) / TSCAN;
+      if ((rc = ws.row_count.ensure((size_t)n_rows * 4 + 16)) || (rc = ws.row_lexcl.ensure((size_t)n_rows * 8 + 16)) ||
+          (rc = ws.row_bsum.ensure((size_t)n_blk * 8 + 16)))
+        return rc;
+      if (n_rows) {
+        dense_count_kernel<<<(n_rows + 255) / 256, 256, 0, st>>>(ws.row_ptr.as<uint64_t>(), n_rows, dq->pairs() ? 1u : 0u, budget, dq->pairs() ? P.strategy : 0u, dq->stride,
+                                                               n_special, ws.row_count.as<uint32_t>(), &ctl->max_all, &ctl->err, &ctl->stride_m);
+        tile_scan_block_kernel<<<(unsigned)n_blk, TSCAN, 0, st>>>(ws.row_count.as<uint32_t>(), ws.row_lexcl.as<unsigned long long>(),
+                                                                 ws.row_bsum.as<unsigned long long>(), n_rows);
+        tile_scan_top_kernel<<<1, TSCAN, 0, st>>>(ws.row_bsum.as<unsigned long long>(), n_blk, &ctl->rows);
+        e->last_launches += 3;
+      }
+      rec(e, st, "dense_count");
+    } else {
+      if (!dq->batch_longest && (rc = launch_dense(e, ws, n_rows, n_rows, *dq, st))) return rc;
+      rec(e, st, dq->pairs() ? "dense_pair_rows" : "dense_rows");
+    }
   }
   CU(cudaMemcpyAsync(ws.h_ctl.p, ws.ctl.p, sizeof(ctl_block), cudaMemcpyDeviceToHost, st));
   return B2T_OK;
@@ -793,6 +896,9 @@ static int check_run(b2t_engine* e, Workspace& ws, cudaStream_t st, bool* reran 
     if ((c->err | c->lc.err) & ERR_INTERNAL) return fail(B2T_ERR_CUDA, "internal error: long pre-token / added-token bookkeeping mismatch");
     if (!(c->lc.err & ERR_POOL_OVERFLOW)) {
       if (c->err & ERR_TRUNCATION) return fail(B2T_ERR_TRUNCATION, "Truncation error: Sequence to truncate too short to respect the provided max_length");
+      if (c->err & ERR_STRIDE)
+        return fail(B2T_ERR_TRUNCATION, "`stride` must be strictly less than `max_len=%u` (note that `max_len` may be shorter than the max length of the "
+                    "original model, as it subtracts the number of special characters", c->stride_m);
       return B2T_OK;
     }
     if (attempt >= 2) return fail(B2T_ERR_CUDA, "long pool did not converge");
@@ -845,6 +951,7 @@ static int device_encode(const char* fn, b2t_engine* e, const void* out, const u
   if (((uintptr_t)d_bytes & 15u) != 0) return fail(B2T_ERR_INVALID, "%s: d_bytes must be 16-byte aligned", fn);
   int rc;
   if (dq && (rc = make_dense_req(spec, dq))) return rc;
+  if (dq && dq->offsets) flags |= B2T_WANT_OFFSETS;   // offset rows come from the CSR's offsets
   std::lock_guard<std::mutex> lk(e->dev_mu);
   CU(cudaSetDevice(e->device));
   cudaStream_t st = stream ? (cudaStream_t)stream : e->own_stream;
@@ -962,6 +1069,17 @@ extern "C" int b2t_engine_set_added_tokens(b2t_engine* e, uint32_t n_tokens, con
 }
 
 // ------------------------------------------------------------------------------------------------ dense mode
+// After a dense run with overflowing parts: the rows it makes (*n_rows; `before` rows precede them in the result) and
+// whether they all fit L
+static int overflow_rows(const ctl_block* c, uint64_t before, uint32_t L, uint32_t* n_rows) {
+  if (before + c->rows >= (1ull << 31))
+    return fail(B2T_ERR_TOO_LARGE, "the batch makes %llu dense rows or more: at most 2^31 - 1 fit one result", (unsigned long long)(before + c->rows));
+  if (c->max_all > L)
+    return fail(B2T_ERR_INVALID, "an overflowing row of %u tokens does not fit the dense length %u (the reference returns a longer, unpadded row here)", c->max_all, L);
+  *n_rows = (uint32_t)c->rows;
+  return B2T_OK;
+}
+
 extern "C" int b2t_encode_batch_dense(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, const b2t_dense_spec* spec,
                                       b2t_result** out);
 
@@ -973,15 +1091,19 @@ static int dense_device(const char* fn, b2t_engine* e, const uint8_t* d_bytes, u
   return device_encode(fn, e, out, d_bytes, n_bytes, d_doc_off, n_docs, 0u, RUN_RESULT, spec, &dq, stream,
                        [&](Workspace& ws, cudaStream_t st) -> int {
     int rc2;
-    const uint32_t max_row = ws.h_ctl.as<ctl_block>()->max_row, n_rows = n_docs / dq.docs_per_row;
-    if (dq.batch_longest) {
-      dq.L() = dense_round(max_row, dq.multiple);
-      if ((rc2 = launch_dense(e, ws, n_rows, dq, st))) return rc2;   // asynchronous on st, like the CSR entry point's result
-    } else if (max_row > dq.L()) {
+    const ctl_block* c = ws.h_ctl.as<ctl_block>();
+    const uint32_t max_row = c->max_row, n_in = n_docs / dq.docs_per_row;
+    uint32_t n_rows = n_in;
+    if (dq.batch_longest) dq.L() = dense_round(max_row, dq.multiple);
+    else if (max_row > dq.L())
       return fail(B2T_ERR_INVALID, "a row of %u tokens does not fit the dense length %u: enable truncation (the reference returns a longer row here)", max_row, dq.L());
-    }
+    if (dq.overflow && (rc2 = overflow_rows(c, 0, dq.L(), &n_rows))) return rc2;
+    // asynchronous on st, like the CSR entry point's result (a fixed length without overflowing parts: queued already)
+    if ((dq.batch_longest || dq.overflow) && (rc2 = launch_dense(e, ws, n_in, n_rows, dq, st))) return rc2;
     b2t_result* r = new b2t_result();
-    r->eng = e; r->on_device = 1; r->n_docs = n_rows;
+    r->eng = e; r->on_device = 1; r->n_docs = n_in; r->n_rows = n_rows;
+    r->row_sample = dq.overflow ? ws.row_sample.as<uint32_t>() : nullptr;
+    r->dense_off = dq.offsets ? ws.dense_off.as<uint32_t>() : nullptr;
     r->n_tokens = ws.h_ctl.as<ctl_block>()->total;
     r->dense_len = dq.L();
     r->dense_ids = ws.dense_ids.as<uint32_t>(); r->row_len = ws.dense_len.as<uint32_t>();
@@ -1015,7 +1137,11 @@ extern "C" int b2t_encode_pairs_dense_device(b2t_engine* e, const uint8_t* d_byt
 // ------------------------------------------------------------------------------------------------ host pipeline
 static b2t_result* pool_get(b2t_engine* e) {
   std::lock_guard<std::mutex> lk(e->mu);
-  if (!e->pool.empty()) { b2t_result* r = e->pool.back().release(); e->pool.pop_back(); r->type_ids = nullptr; return r; }
+  if (!e->pool.empty()) {
+    b2t_result* r = e->pool.back().release(); e->pool.pop_back();
+    r->type_ids = nullptr; r->n_rows = 0; r->row_sample = nullptr; r->dense_off = nullptr;
+    return r;
+  }
   return new b2t_result();
 }
 
@@ -1064,8 +1190,10 @@ static int queue_dense_copy(b2t_result* r, const Workspace& ws, uint32_t r0, uin
     CU(cudaMemcpyAsync(r->h_dense_ids.as<uint32_t>() + (size_t)r0 * L, ws.dense_ids.p, (size_t)nr * L * 4, cudaMemcpyDeviceToHost, ws.stream));
     if (dq.want_mask) CU(cudaMemcpyAsync(r->h_dense_mask.as<uint8_t>() + (size_t)r0 * L, ws.dense_mask.p, (size_t)nr * L, cudaMemcpyDeviceToHost, ws.stream));
     if (dq.pairs()) CU(cudaMemcpyAsync(r->h_type_ids.as<uint8_t>() + (size_t)r0 * L, ws.dense_type.p, (size_t)nr * L, cudaMemcpyDeviceToHost, ws.stream));
+    if (dq.offsets) CU(cudaMemcpyAsync(r->h_dense_off.as<uint32_t>() + (size_t)r0 * L * 2, ws.dense_off.p, (size_t)nr * L * 8, cudaMemcpyDeviceToHost, ws.stream));
   }
   if (nr) CU(cudaMemcpyAsync(r->h_row_len.as<uint32_t>() + r0, ws.dense_len.p, (size_t)nr * 4, cudaMemcpyDeviceToHost, ws.stream));
+  if (nr && dq.overflow) CU(cudaMemcpyAsync(r->h_row_sample.as<uint32_t>() + r0, ws.row_sample.p, (size_t)nr * 4, cudaMemcpyDeviceToHost, ws.stream));
   return B2T_OK;
 }
 
@@ -1077,7 +1205,7 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
   uint64_t max_chunk = 0;
   DenseReq dq_local;
   DenseReq* dq = nullptr;
-  if (dq_in) { dq_local = *dq_in; dq = &dq_local; flags = 0; }
+  if (dq_in) { dq_local = *dq_in; dq = &dq_local; flags = dq->offsets ? B2T_WANT_OFFSETS : 0u; }   // (offset rows: from the CSR's offsets)
   // BatchLongest padding needs every row length before the first row can be written: the batch runs as one chunk
   if (dq && dq->batch_longest && total_bytes + n_docs >= (1ull << 31))
     return fail(B2T_ERR_UNSUPPORTED, "dense output padded to the longest row needs the batch in one device pass (< 2^31 bytes); pad to a fixed length instead");
@@ -1101,7 +1229,7 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
   b2t_result* r = pool_get(e);
   r->eng = e; r->on_device = 0; r->n_docs = dq ? n_rows : n_docs; r->n_tokens = 0;
   int rc;
-  const bool want_off = (flags & B2T_WANT_OFFSETS) != 0, want_wid = (flags & B2T_WANT_WORD_IDS) != 0;
+  const bool want_off = !dq && (flags & B2T_WANT_OFFSETS) != 0, want_wid = (flags & B2T_WANT_WORD_IDS) != 0;
   // initial capacity guess: 0.30 tokens per byte, grown on demand (pinned pool => steady state allocates nothing)
   uint64_t cap_tok = std::max<uint64_t>(total_bytes * 3 / 10 + 1024, 4096);
   if ((rc = r->h_row_ptr.ensure(((size_t)n_docs + 1) * 8, false))) { pool_put(e, r); return rc; }
@@ -1113,15 +1241,19 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     return B2T_OK;
   };
   r->dense_len = 0; r->dense_ids = nullptr; r->dense_mask = nullptr; r->row_len = nullptr; r->type_ids = nullptr;
-  auto dense_host = [&](uint32_t L) -> int {   // pinned rows of the whole batch
+  // pinned rows: the whole batch's n_rows rows, or with overflowing parts a guess grown on demand (contents kept)
+  uint64_t cap_rows = 0, row_total = 0;
+  auto dense_host = [&](uint32_t L, uint64_t rows, bool keep) -> int {
     int rc2;
-    const size_t cells = (size_t)n_rows * L;
-    if ((rc2 = r->h_dense_ids.ensure(cells * 4 + 16, false)) || (rc2 = r->h_row_len.ensure((size_t)n_rows * 4 + 16, false)) ||
-        (dq->want_mask && (rc2 = r->h_dense_mask.ensure(cells + 16, false))) || (dq->pairs() && (rc2 = r->h_type_ids.ensure(cells + 16, false))))
+    const size_t cells = (size_t)rows * L;
+    if ((rc2 = r->h_dense_ids.ensure(cells * 4 + 16, keep)) || (rc2 = r->h_row_len.ensure((size_t)rows * 4 + 16, keep)) ||
+        (dq->want_mask && (rc2 = r->h_dense_mask.ensure(cells + 16, keep))) || (dq->pairs() && (rc2 = r->h_type_ids.ensure(cells + 16, keep))) ||
+        (dq->overflow && (rc2 = r->h_row_sample.ensure((size_t)rows * 4 + 16, keep))) || (dq->offsets && (rc2 = r->h_dense_off.ensure(cells * 8 + 16, keep))))
       return rc2;
+    cap_rows = rows;
     return B2T_OK;
   };
-  if (dq) { if (!dq->batch_longest && (rc = dense_host(dq->L()))) { pool_put(e, r); return rc; } }
+  if (dq) { if (!dq->batch_longest && (rc = dense_host(dq->L(), n_rows, false))) { pool_put(e, r); return rc; } }
   else if ((rc = grow(cap_tok))) { pool_put(e, r); return rc; }
 
   uint64_t tok_base = 0;
@@ -1139,15 +1271,29 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     const uint64_t nt = ws.h_ctl.as<ctl_block>()->total;
     c.tok_base = tok_base;
     if (dq) {
-      const uint32_t nr = (c.d1 - c.d0) / per, max_row = ws.h_ctl.as<ctl_block>()->max_row;
+      const ctl_block* cb = ws.h_ctl.as<ctl_block>();
+      const uint32_t n_in = (c.d1 - c.d0) / per, max_row = cb->max_row;
+      uint32_t nr = n_in;
       if (dq->batch_longest) {   // one chunk: L is known now
         dq->L() = dense_round(max_row, dq->multiple);
-        if ((rc2 = dense_host(dq->L())) || (rc2 = launch_dense(e, ws, nr, *dq, ws.stream))) return rc2;
+        if (!dq->overflow && (rc2 = dense_host(dq->L(), n_rows, false))) return rc2;
       } else if (max_row > dq->L()) {
         return fail(B2T_ERR_INVALID, "a row of %u tokens does not fit the dense length %u: enable truncation (the reference returns a longer row here)", max_row, dq->L());
       }
-      // (a fixed length: the rows were queued for the copy right behind the kernels, see issue(); a rerun has replaced them)
-      if ((dq->batch_longest || reran) && (rc2 = queue_dense_copy(r, ws, c.d0 / per, nr, *dq))) return rc2;
+      if (dq->overflow) {
+        // the chunk's rows go at the running row base; earlier chunks may still be copying into the old buffers: let them
+        // land, then grow (contents are kept)
+        if ((rc2 = overflow_rows(cb, row_total, dq->L(), &nr))) return rc2;
+        if (row_total + nr > cap_rows) {
+          for (auto& s : ss.slot) if (s.stream) CU(cudaStreamSynchronize(s.stream));
+          if ((rc2 = dense_host(dq->L(), std::max<uint64_t>((row_total + nr) * 2, (uint64_t)n_rows), true))) return rc2;
+        }
+      }
+      if ((dq->batch_longest || dq->overflow) && (rc2 = launch_dense(e, ws, n_in, nr, *dq, ws.stream, c.d0 / per))) return rc2;
+      // (a fixed length without overflowing parts: the rows were queued for the copy right behind the kernels, see issue();
+      // a rerun has replaced them)
+      if ((dq->batch_longest || dq->overflow || reran) && (rc2 = queue_dense_copy(r, ws, (uint32_t)row_total, nr, *dq))) return rc2;
+      row_total += nr;
       tok_base += nt;
       return B2T_OK;
     }
@@ -1189,7 +1335,7 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     if ((rc2 = run_device_pipeline(e, ws, ws.stream))) return rc2;
     // dense rows of a fixed length: their place in the result does not depend on anything the host has to read first, so
     // the copy back is queued right behind the kernels (the CSR modes need the chunk's token count for that)
-    if (dq && !dq->batch_longest && (rc2 = queue_dense_copy(r, ws, c.d0 / per, nd / per, *dq))) return rc2;
+    if (dq && !dq->batch_longest && !dq->overflow && (rc2 = queue_dense_copy(r, ws, c.d0 / per, nd / per, *dq))) return rc2;
     CU(cudaEventRecord(ws.done, ws.stream));
     return B2T_OK;
   };
@@ -1211,6 +1357,9 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     r->dense_ids = r->h_dense_ids.as<uint32_t>(); r->row_len = r->h_row_len.as<uint32_t>();
     r->dense_mask = dq->want_mask ? r->h_dense_mask.as<uint8_t>() : nullptr;
     r->type_ids = dq->pairs() ? r->h_type_ids.as<uint8_t>() : nullptr;
+    r->n_rows = (uint32_t)row_total;
+    r->row_sample = dq->overflow ? r->h_row_sample.as<uint32_t>() : nullptr;
+    r->dense_off = dq->offsets ? r->h_dense_off.as<uint32_t>() : nullptr;
   } else {
     // chunk-relative row_ptr -> batch-relative (host fix-up: one addition per document)
     uint64_t* rp = r->h_row_ptr.as<uint64_t>();
@@ -1342,6 +1491,9 @@ extern "C" const uint32_t* b2t_result_dense_ids(const b2t_result* r) { return r 
 extern "C" const uint8_t* b2t_result_attention_mask(const b2t_result* r) { return r ? r->dense_mask : nullptr; }
 extern "C" const uint32_t* b2t_result_row_lengths(const b2t_result* r) { return r ? r->row_len : nullptr; }
 extern "C" const uint8_t* b2t_result_type_ids(const b2t_result* r) { return r ? r->type_ids : nullptr; }
+extern "C" uint32_t b2t_result_dense_rows(const b2t_result* r) { return r ? r->n_rows : 0; }
+extern "C" const uint32_t* b2t_result_row_sample(const b2t_result* r) { return r ? r->row_sample : nullptr; }
+extern "C" const uint32_t* b2t_result_dense_offsets(const b2t_result* r) { return r ? r->dense_off : nullptr; }
 extern "C" void b2t_result_free(b2t_result* r) {
   if (!r) return;
   if (r->on_device || !r->eng) { delete r; return; }
