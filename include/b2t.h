@@ -153,8 +153,21 @@ enum {
   B2T_DENSE_OVERFLOW = 1u,  /* return_overflowing_tokens: every part Encoding::truncate makes (tokenizer/encoding.rs:307-388) is a
                                row -- an input's kept row first, then its overflowing rows (`[e] + e.overflowing`), each with the
                                template around it; b2t_result_row_sample maps each row to its input */
-  B2T_DENSE_OFFSETS = 2u    /* return_offsets_mapping: [rows, L] (start, end) char offsets relative to the row's sequence
+  B2T_DENSE_OFFSETS = 2u,   /* return_offsets_mapping: [rows, L] (start, end) char offsets relative to the row's sequence
                                (growing_offsets = false), (0, 0) for special tokens and padding */
+  B2T_DENSE_TRIM_OFFSETS = 4u,  /* trim_offsets (pre_tokenizers/byte_level.rs:202-234 process_offsets, on every part of every
+                                   sequence): the offset rows skip a token's leading / trailing U+0120 or whitespace chars --
+                                   of its vocabulary string, or for an added token of the span it matched.  Needs
+                                   B2T_DENSE_OFFSETS (else B2T_ERR_INVALID) and a BPE engine (else B2T_ERR_UNSUPPORTED).  An
+                                   added token with both lstrip and rstrip that absorbed whitespace in a row fails the call
+                                   with B2T_ERR_UNSUPPORTED: which side the whitespace came from is not in its offsets. */
+  B2T_DENSE_TRIM_PREFIX_SPACE = 8u,  /* the post-processor's add_prefix_space: a part's first token (or one at offset 0) keeps a
+                                        single leading space.  Only with B2T_DENSE_TRIM_OFFSETS. */
+  B2T_DENSE_SPECIAL_MASK = 16u,  /* special_tokens_mask: [rows, L] u8, 1 for template tokens and padding (encoding.rs:465-519) */
+  B2T_DENSE_SEQUENCE_IDS = 32u,  /* sequence ids: [rows, L] i8, 0 for A's tokens, 1 for B's, -1 (None) for template tokens and
+                                    padding (encoding.rs:137-145) */
+  B2T_DENSE_WORD_IDS = 64u       /* word ids: [rows, L] u32, the word of every sequence token (restarting per sequence),
+                                    0xFFFFFFFF (None) for template tokens and padding */
 };
 typedef struct {
   uint32_t struct_size;        /* sizeof(b2t_dense_spec) */
@@ -194,6 +207,9 @@ const uint32_t* b2t_result_row_lengths(const b2t_result* r);  /* R */
 const uint32_t* b2t_result_row_sample(const b2t_result* r);   /* R: the input of each row (overflow_to_sample_mapping), or NULL
                                                                  without B2T_DENSE_OVERFLOW */
 const uint32_t* b2t_result_dense_offsets(const b2t_result* r); /* R * L * 2 (start, end), or NULL without B2T_DENSE_OFFSETS */
+const uint8_t* b2t_result_special_tokens_mask(const b2t_result* r); /* R * L, or NULL without B2T_DENSE_SPECIAL_MASK */
+const int8_t* b2t_result_sequence_ids(const b2t_result* r);          /* R * L, or NULL without B2T_DENSE_SEQUENCE_IDS */
+const uint32_t* b2t_result_dense_word_ids(const b2t_result* r);      /* R * L, or NULL without B2T_DENSE_WORD_IDS */
 
 /* Dense mode for PAIRS of sequences (EncodeInput::Dual): what the reference runs after the path for a batch of pairs --
  * truncate_encodings with a pair (utils/truncation.rs:70-162, kept parts only), the pair template (processors/template.rs:

@@ -13,6 +13,7 @@ ADDED_SINGLE_WORD, ADDED_LSTRIP, ADDED_RSTRIP, ADDED_NORMALIZED = 1, 2, 4, 8
 TRUNC_LONGEST_FIRST, TRUNC_ONLY_FIRST, TRUNC_ONLY_SECOND = 0, 1, 2
 PIECE_A, PIECE_B = 0x80000000, 0x80000001
 DENSE_OVERFLOW, DENSE_OFFSETS = 1, 2
+DENSE_TRIM_OFFSETS, DENSE_TRIM_PREFIX_SPACE, DENSE_SPECIAL_MASK, DENSE_SEQUENCE_IDS, DENSE_WORD_IDS = 4, 8, 16, 32, 64
 
 # every symbol include/b2t.h declares
 SYMBOLS = ["b2t_engine_create", "b2t_engine_destroy", "b2t_engine_set_added_tokens", "b2t_encode_batch", "b2t_encode_batch_device", "b2t_encode_batch_device_begin",
@@ -21,6 +22,7 @@ SYMBOLS = ["b2t_engine_create", "b2t_engine_destroy", "b2t_engine_set_added_toke
            "b2t_result_attention_mask", "b2t_result_row_lengths",
            "b2t_encode_pairs_dense", "b2t_encode_pairs_dense_device", "b2t_result_type_ids",
            "b2t_result_dense_rows", "b2t_result_row_sample", "b2t_result_dense_offsets",
+           "b2t_result_special_tokens_mask", "b2t_result_sequence_ids", "b2t_result_dense_word_ids",
            "b2t_result_n_tokens", "b2t_result_n_docs", "b2t_result_on_device", "b2t_result_ids", "b2t_result_offsets",
            "b2t_result_word_ids", "b2t_result_row_ptr", "b2t_result_free", "b2t_host_alloc", "b2t_host_free",
            "b2t_engine_set_profiling", "b2t_engine_last_kernels", "b2t_unicode_class_table", "b2t_bert_normalizer_images", "b2t_last_error", "b2t_version"]
@@ -89,7 +91,7 @@ def lib():
     L.b2t_encode_pairs_dense_device.argtypes = [vp, vp, u64, vp, u32, ctypes.POINTER(PairDenseSpec), vp, ctypes.POINTER(vp)]
     L.b2t_result_dense_rows.argtypes = [vp]; L.b2t_result_dense_rows.restype = u32
     for f in ("b2t_result_dense_ids", "b2t_result_attention_mask", "b2t_result_row_lengths", "b2t_result_type_ids", "b2t_result_row_sample",
-              "b2t_result_dense_offsets"):
+              "b2t_result_dense_offsets", "b2t_result_special_tokens_mask", "b2t_result_sequence_ids", "b2t_result_dense_word_ids"):
         getattr(L, f).argtypes = [vp]; getattr(L, f).restype = vp
     L.b2t_result_n_tokens.argtypes = [vp]; L.b2t_result_n_tokens.restype = u64
     L.b2t_result_n_docs.argtypes = [vp]; L.b2t_result_n_docs.restype = u32

@@ -91,15 +91,88 @@ struct DenseOverflow {
   uint2* out_off;                // [rows, L] offsets, (0, 0) for special tokens and padding
 };
 
+// ------------------------------------------------------------------------------------------------- row metadata
+// The per-position fields of the reference's post-processed Encoding besides ids, type ids and offsets: the special-tokens
+// mask (encoding.rs:465-519: 1 for template tokens and padding), sequence ids (encoding.rs:137-145: None for those, A's
+// tokens 0 and B's 1 whatever the template order), word ids (the CSR's, None for those) -- and offset trimming:
+//   pre_tokenizers/byte_level.rs:202-234  process_offsets, run on every part of every sequence after truncation and before
+//                                         the template (roberta.rs:71-79, byte_level.rs:180-193)
+enum { ERR_TRIM_AMBIGUOUS = 128u };   // ctl err bit: an lstrip + rstrip added token absorbed whitespace (added_trim_counts)
+enum { TRIM_ALL_SPACE = 1u, TRIM_LSTRIP = 2u, TRIM_RSTRIP = 4u };
+
+// process_offsets on one token's offsets o: ld / tr = its leading / trailing chars that are U+0120 or whitespace.  The
+// start moves past ld, except that with the post-processor's add_prefix_space (aps) a first token of its part (`first`)
+// or one at offset 0 keeps a single leading space; the end moves back by tr where o1 >= tr, never before the new start.
+__host__ __device__ inline uint2 trim_span(uint2 o, uint32_t ld, uint32_t tr, bool first, bool aps) {
+  const bool keep = (first || o.x == 0u) && aps && ld == 1u;
+  const uint32_t n0 = ld > 0u && !keep ? (o.x + ld < o.y ? o.x + ld : o.y) : o.x;
+  const uint32_t n1 = tr > 0u && o.y >= tr ? (o.y - tr > n0 ? o.y - tr : n0) : o.y;
+  return make_uint2(n0, n1);
+}
+
+// An added token as process_offsets sees it: its text is the span it matched, content plus the whitespace lstrip / rstrip
+// absorbed (tokenizer.py _span_spaces).  counts = leading | trailing << 16 whitespace-or-U+0120 chars of the content.
+struct AddedTrim { uint32_t id, chars, counts, flags; };   // flags: TRIM_*
+
+// The counts of an occurrence whose span is S chars long (o1 - o0).  The S - chars absorbed chars lie left of the content
+// for lstrip alone, right of it for rstrip alone.  false: both flags and S > chars -- how the absorbed whitespace splits
+// between the two sides is not in the offsets.
+__host__ __device__ inline bool added_trim_counts(uint32_t S, const AddedTrim& a, uint32_t* ld, uint32_t* tr) {
+  const bool l = (a.flags & TRIM_LSTRIP) != 0u, r = (a.flags & TRIM_RSTRIP) != 0u;
+  const uint32_t extra = S > a.chars ? S - a.chars : 0u;
+  if (l && r && extra) return false;
+  if (a.flags & TRIM_ALL_SPACE) { *ld = S; *tr = S; return true; }
+  *ld = (l ? extra : 0u) + (a.counts & 0xFFFFu);
+  *tr = (r ? extra : 0u) + (a.counts >> 16);
+  return true;
+}
+
+// What the META instantiations of the row kernels read and write besides the spec.  Null output = not asked for.
+struct DenseMeta {
+  const uint32_t* trim_vocab;    // per vocabulary id: leading | trailing << 16 whitespace-or-U+0120 chars; null = no trimming
+  const AddedTrim* trim_added;   // the added tokens by ascending id (their CSR ids carry bit 31)
+  uint32_t n_added, aps;         // aps: the post-processor's add_prefix_space
+  const uint32_t* word_ids;      // the CSR's word ids (out_word)
+  uint8_t* out_special; int8_t* out_seq; uint32_t* out_word;   // [rows, L]
+  uint32_t* err;                 // ERR_TRIM_AMBIGUOUS, ERR_INTERNAL_META
+};
+enum { ERR_INTERNAL_META = 4u };   // (long_kernels.cuh ERR_INTERNAL: a marked id that is no added token)
+
+// the offsets of sequence token `id` (a CSR id: bit 31 = added token), trimmed when M asks for it
+__device__ __forceinline__ uint2 meta_offsets(const DenseMeta& M, uint32_t id, uint2 o, bool first) {
+  if (!M.trim_vocab) return o;
+  uint32_t ld, tr;
+  if (id >> 31) {
+    uint32_t lo = 0, hi = M.n_added;
+    const uint32_t want = id & 0x7FFFFFFFu;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (M.trim_added[mid].id < want) lo = mid + 1; else hi = mid; }
+    if (lo == M.n_added || M.trim_added[lo].id != want) { atomicOr(M.err, (unsigned)ERR_INTERNAL_META); return o; }
+    if (!added_trim_counts(o.y - o.x, M.trim_added[lo], &ld, &tr)) { atomicOr(M.err, (unsigned)ERR_TRIM_AMBIGUOUS); return o; }
+  } else {
+    const uint32_t c = M.trim_vocab[id];
+    ld = c & 0xFFFFu; tr = c >> 16;
+  }
+  return trim_span(o, ld, tr, first, M.aps != 0u);
+}
+
+// cell `cell` of the metadata rows: a sequence token of sequence `seq` at CSR position t, or (tok false) a template token
+// or padding
+__device__ __forceinline__ void meta_write(const DenseMeta& M, size_t cell, bool tok, uint32_t seq, uint64_t t) {
+  if (M.out_special) M.out_special[cell] = tok ? 0 : 1;
+  if (M.out_seq) M.out_seq[cell] = tok ? (int8_t)seq : (int8_t)-1;
+  if (M.out_word) M.out_word[cell] = tok ? M.word_ids[t] : 0xFFFFFFFFu;
+}
+
 // One warp per row.  row_ptr is the (chunk-relative) CSR of `ids`; rows are written at out_* + d * L.
 // A row that does not fit L (padding to a fixed length without truncation) raises bit 0 of *err and is cut -- the host
 // turns that into an error, the reference would return a longer row there.
 // OVER: n_docs counts rows, each the template around one part of its input (the host has checked that every row fits
-// L); OFFS: the offset rows as well.
-template <bool OVER = false, bool OFFS = false>
+// L); OFFS: the offset rows as well; META: the rows of DenseMeta (trimmed offsets, ids without the added-token mark), the
+// part's first token at position n_pre.
+template <bool OVER = false, bool OFFS = false, bool META = false>
 __global__ void dense_rows_kernel(const uint32_t* __restrict__ ids, const uint64_t* __restrict__ row_ptr, uint32_t n_docs, const DenseSpec S,
                                   uint32_t* __restrict__ out_ids, uint8_t* __restrict__ out_mask, uint32_t* __restrict__ out_len,
-                                  uint32_t* __restrict__ err, const DenseOverflow O = DenseOverflow{}) {
+                                  uint32_t* __restrict__ err, const DenseOverflow O = DenseOverflow{}, const DenseMeta M = DenseMeta{}) {
   const uint32_t d = (uint32_t)(((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
   const int lane = threadIdx.x & 31;
   if (d >= n_docs) return;
@@ -127,9 +200,23 @@ __global__ void dense_rows_kernel(const uint32_t* __restrict__ ids, const uint64
       else if (k < S.n_pre + keep) v = ids[src + (k - S.n_pre)];
       else v = S.post[k - S.n_pre - keep];
     }
-    row[j] = v;
-    if (mrow) mrow[j] = k < len ? 1 : 0;
-    if constexpr (OFFS) O.out_off[(size_t)d * S.L + j] = k >= S.n_pre && k < S.n_pre + keep ? O.offsets[src + (k - S.n_pre)] : make_uint2(0u, 0u);
+    if constexpr (META) {
+      const bool tok = k >= S.n_pre && k < S.n_pre + keep;
+      const uint64_t t = src + (k - S.n_pre);
+      uint2 o = make_uint2(0u, 0u);
+      if (tok) {
+        if constexpr (OFFS) o = meta_offsets(M, v, O.offsets[t], k == S.n_pre);
+        v &= 0x7FFFFFFFu;
+      }
+      row[j] = v;
+      if (mrow) mrow[j] = k < len ? 1 : 0;
+      if constexpr (OFFS) O.out_off[(size_t)d * S.L + j] = o;
+      meta_write(M, (size_t)d * S.L + j, tok, 0u, t);
+    } else {
+      row[j] = v;
+      if (mrow) mrow[j] = k < len ? 1 : 0;
+      if constexpr (OFFS) O.out_off[(size_t)d * S.L + j] = k >= S.n_pre && k < S.n_pre + keep ? O.offsets[src + (k - S.n_pre)] : make_uint2(0u, 0u);
+    }
   }
   if (lane == 0 && out_len) out_len[d] = len;
 }
@@ -200,11 +287,13 @@ __global__ void pair_len_max_kernel(const uint64_t* __restrict__ row_ptr, uint32
 // out_* + p * L.  A row that does not fit L is left unwritten: the host has found it through pair_len_max_kernel and
 // fails the batch.  The spec is read in place (__grid_constant__), so the special-token look-up needs no local copy.
 // OVER: one warp per row, row p merging part i of X with part j of Y (pair_row_part) -- a kept part takes its piece's
-// type id, an overflowing one O.type_ox / O.type_oy; OFFS: the offset rows as well.
-template <bool OVER = false, bool OFFS = false>
+// type id, an overflowing one O.type_ox / O.type_oy; OFFS: the offset rows as well; META: the rows of DenseMeta, X's and
+// Y's parts each with its own first token (positions e0 and e2), X's tokens of sequence b_first and Y's of the other.
+template <bool OVER = false, bool OFFS = false, bool META = false>
 __global__ void dense_pair_rows_kernel(const uint32_t* __restrict__ ids, const uint64_t* __restrict__ row_ptr, uint32_t n_pairs,
                                        const __grid_constant__ PairDenseSpec S, uint32_t* __restrict__ out_ids, uint8_t* __restrict__ out_type,
-                                       uint8_t* __restrict__ out_mask, uint32_t* __restrict__ out_len, const __grid_constant__ DenseOverflow O = DenseOverflow{}) {
+                                       uint8_t* __restrict__ out_mask, uint32_t* __restrict__ out_len, const __grid_constant__ DenseOverflow O = DenseOverflow{},
+                                       const __grid_constant__ DenseMeta M = DenseMeta{}) {
   const uint32_t p = (uint32_t)(((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
   const int lane = threadIdx.x & 31;
   if (p >= n_pairs) return;
@@ -250,6 +339,15 @@ __global__ void dense_pair_rows_kernel(const uint32_t* __restrict__ ids, const u
     } else if (k < e3) {
       v = ids[src_y + (k - e2)]; t = type_y;
       if constexpr (OFFS) o = O.offsets[src_y + (k - e2)];
+    }
+    if constexpr (META) {
+      const bool in_x = k >= e0 && k < e1, tok = in_x || (k >= e2 && k < e3);
+      const uint64_t at = in_x ? src_x + (k - e0) : src_y + (k - e2);
+      if (tok) {
+        if constexpr (OFFS) o = meta_offsets(M, v, o, k == (in_x ? e0 : e2));
+        v &= 0x7FFFFFFFu;
+      }
+      meta_write(M, (size_t)p * S.L + j, tok, in_x == (S.b_first != 0u) ? 1u : 0u, at);
     }
     row[j] = v;
     trow[j] = (uint8_t)t;

@@ -130,7 +130,10 @@ struct DenseReq {
   // overflowing parts (B2T_DENSE_OVERFLOW): rows per input are known after the count pass; offset rows (B2T_DENSE_OFFSETS)
   bool overflow = false, offsets = false;
   uint32_t stride = 0, type_oa = 0, type_ob = 0;
+  // row metadata (B2T_DENSE_TRIM_OFFSETS .. B2T_DENSE_WORD_IDS): the META instantiations of the row kernels
+  bool trim = false, aps = false, special_mask = false, seq_ids = false, word_ids = false;
   bool pairs() const { return docs_per_row == 2; }
+  bool meta() const { return trim || special_mask || seq_ids || word_ids; }
   uint32_t& L() { return pairs() ? P.L : S.L; }
   uint32_t L() const { return pairs() ? P.L : S.L; }
 };
@@ -166,6 +169,7 @@ struct Workspace {
   DevBuf wcache;                      // per-batch word cache (model_kernels.cuh)
   DevBuf dense_ids, dense_mask, dense_len, dense_type;  // dense [n_rows, L] rows (dense_kernels.cuh); type ids: pairs only
   DevBuf dense_off, row_count, row_lexcl, row_bsum, row_base, row_sample;  // overflow rows: offset rows, the count pass and its scan
+  DevBuf dense_special, dense_seq, dense_word;   // row metadata: special-tokens mask, sequence ids, word ids
   // BertNormalizer pre-pass (norm_kernels.cuh): the normalized batch and what maps its tokens back to the original
   DevBuf nrm_doc_bits, nrm_pfd, nrm_page_out, nrm_page_chars, nrm_lexcl_o, nrm_bsum_o, nrm_lexcl_c, nrm_bsum_c, nrm_tot, nrm_bytes, nrm_src_char, nrm_doc_off, nrm_doc_char0;
   bool norm_active = false;
@@ -195,7 +199,8 @@ struct b2t_result {
   const uint8_t* type_ids = nullptr;
   uint32_t n_rows = 0;   // dense rows R (n_docs without overflowing parts)
   const uint32_t* row_sample = nullptr; const uint32_t* dense_off = nullptr;
-  PinBuf h_dense_ids, h_dense_mask, h_row_len, h_type_ids, h_row_sample, h_dense_off;
+  const uint8_t* special_mask = nullptr; const int8_t* seq_ids = nullptr; const uint32_t* dense_word = nullptr;
+  PinBuf h_dense_ids, h_dense_mask, h_row_len, h_type_ids, h_row_sample, h_dense_off, h_special, h_seq, h_word;
 };
 
 constexpr int NSLOT = 3;   // chunk workspaces of one host-path call: NSLOT - 1 chunks are in flight while the next is issued
@@ -217,6 +222,10 @@ struct b2t_engine {
   int has_added = 0;
   AddedTables at;
   DevBuf d_at_bytes, d_at_off, d_at_id, d_at_flags, d_at_first, d_at_pair, d_cls_rust;
+  // offset trimming in dense rows (BPE engines): per vocabulary id / per added token (dense_kernels.cuh DenseMeta)
+  DevBuf d_trim_vocab, d_trim_added;
+  uint32_t n_trim_added = 0;
+  int trim_ready = 0, added_both = 0;   // added_both: an added token has lstrip and rstrip (the rows may refuse it)
   // Concurrency: the tables are immutable, every host-path call (b2t_encode_batch, _dense, b2t_pre_tokenize_batch) runs on a
   // slot set of its own -- NSLOT workspaces with their streams -- so calls from several host threads overlap their copies
   // and kernels; `mu` only guards the pools (and the whole call while per-kernel profiling is on: the event records are one
@@ -332,6 +341,10 @@ extern "C" int b2t_engine_create(const b2t_config* cfg, b2t_engine** out) {
   // (the merge-table probes of the merge rounds are read-only loads and hit there)
   cudaFuncSetAttribute(model_tile_kernel<MODEL_BPE>, cudaFuncAttributePreferredSharedMemoryCarveout, 86);
   cudaFuncSetAttribute(model_tile_kernel<MODEL_WORDPIECE>, cudaFuncAttributePreferredSharedMemoryCarveout, 86);
+  if (cfg->model == B2T_MODEL_BPE) {   // (the ByteLevel pre-tokenizers: the only ones BPE runs behind)
+    if ((rc = upload(e->d_trim_vocab, vocab_trim_counts(cfg->n_vocab, cfg->vocab_bytes, cfg->vocab_off, cfg->vocab_ids)))) return rc;
+    e->trim_ready = 1;
+  }
   cudaError_t se = cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking);
   if (se != cudaSuccess) return fail(B2T_ERR_CUDA, "cudaStreamCreate failed: %s", cudaGetErrorString(se));
   *out = e.release();
@@ -429,9 +442,24 @@ static bool read_spec(const Spec* sp, Spec* out) {
 static_assert(offsetof(b2t_dense_spec, stride) == 60 && offsetof(b2t_pair_dense_spec, stride) == 60, "the specs' first layout was 64 bytes");
 
 static int dense_flags(uint32_t flags, uint32_t stride, DenseReq* dq) {
-  if (flags & ~(uint32_t)(B2T_DENSE_OVERFLOW | B2T_DENSE_OFFSETS)) return fail(B2T_ERR_INVALID, "unknown dense_flags 0x%x", flags);
+  constexpr uint32_t known = B2T_DENSE_OVERFLOW | B2T_DENSE_OFFSETS | B2T_DENSE_TRIM_OFFSETS | B2T_DENSE_TRIM_PREFIX_SPACE | B2T_DENSE_SPECIAL_MASK |
+                             B2T_DENSE_SEQUENCE_IDS | B2T_DENSE_WORD_IDS;
+  if (flags & ~known) return fail(B2T_ERR_INVALID, "unknown dense_flags 0x%x", flags);
   dq->overflow = (flags & B2T_DENSE_OVERFLOW) != 0; dq->offsets = (flags & B2T_DENSE_OFFSETS) != 0;
   dq->stride = dq->overflow ? stride : 0u;
+  dq->trim = (flags & B2T_DENSE_TRIM_OFFSETS) != 0; dq->aps = (flags & B2T_DENSE_TRIM_PREFIX_SPACE) != 0;
+  if (dq->trim && !dq->offsets) return fail(B2T_ERR_INVALID, "B2T_DENSE_TRIM_OFFSETS trims offset rows: it needs B2T_DENSE_OFFSETS");
+  if (dq->aps && !dq->trim) return fail(B2T_ERR_INVALID, "B2T_DENSE_TRIM_PREFIX_SPACE is a rule of offset trimming: it needs B2T_DENSE_TRIM_OFFSETS");
+  dq->special_mask = (flags & B2T_DENSE_SPECIAL_MASK) != 0; dq->seq_ids = (flags & B2T_DENSE_SEQUENCE_IDS) != 0;
+  dq->word_ids = (flags & B2T_DENSE_WORD_IDS) != 0;
+  return B2T_OK;
+}
+
+// What a dense request asks of the engine: trimming needs its vocabulary counts (BPE); the CSR flags the run needs for
+// offset rows, word ids and, behind trimming, the added-token marks
+static int dense_engine_flags(const b2t_engine* e, const DenseReq& dq, uint32_t* flags) {
+  if (dq.trim && !e->trim_ready) return fail(B2T_ERR_UNSUPPORTED, "offset trimming (B2T_DENSE_TRIM_OFFSETS) needs a BPE engine behind a ByteLevel pre-tokenizer");
+  *flags = (dq.offsets ? B2T_WANT_OFFSETS : 0u) | (dq.word_ids ? B2T_WANT_WORD_IDS : 0u) | (dq.trim && e->has_added ? B2T_FLAG_ADDED_IDS : 0u);
   return B2T_OK;
 }
 
@@ -515,16 +543,29 @@ static int make_dense_req(const b2t_pair_dense_spec* sp_in, DenseReq* dq) {
   return B2T_OK;
 }
 
-template <bool OVER, bool OFFS>
-static void launch_rows(Workspace& ws, uint32_t n_rows, const DenseReq& dq, const DenseOverflow& O, cudaStream_t st) {
+template <bool OVER, bool OFFS, bool META = false>
+static void launch_rows(Workspace& ws, uint32_t n_rows, const DenseReq& dq, const DenseOverflow& O, cudaStream_t st, const DenseMeta& M = DenseMeta{}) {
   const unsigned grid = (unsigned)(((uint64_t)n_rows * 32 + 255) / 256);
   if (dq.pairs())
-    dense_pair_rows_kernel<OVER, OFFS><<<grid, 256, 0, st>>>(ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.P, ws.dense_ids.as<uint32_t>(),
-                                                             ws.dense_type.as<uint8_t>(), dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr,
-                                                             ws.dense_len.as<uint32_t>(), O);
+    dense_pair_rows_kernel<OVER, OFFS, META><<<grid, 256, 0, st>>>(ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.P, ws.dense_ids.as<uint32_t>(),
+                                                                   ws.dense_type.as<uint8_t>(), dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr,
+                                                                   ws.dense_len.as<uint32_t>(), O, M);
   else
-    dense_rows_kernel<OVER, OFFS><<<grid, 256, 0, st>>>(ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.S, ws.dense_ids.as<uint32_t>(),
-                                                        dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr, ws.dense_len.as<uint32_t>(), nullptr, O);
+    dense_rows_kernel<OVER, OFFS, META><<<grid, 256, 0, st>>>(ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.S, ws.dense_ids.as<uint32_t>(),
+                                                              dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr, ws.dense_len.as<uint32_t>(), nullptr, O, M);
+}
+
+// The row metadata buffers of n_rows rows and what the META row kernels read (ensures the buffers)
+static int make_meta(b2t_engine* e, Workspace& ws, size_t cells, const DenseReq& dq, DenseMeta* M) {
+  int rc;
+  if ((dq.special_mask && (rc = ws.dense_special.ensure(cells + 16))) || (dq.seq_ids && (rc = ws.dense_seq.ensure(cells + 16))) ||
+      (dq.word_ids && (rc = ws.dense_word.ensure(cells * 4 + 16))))
+    return rc;
+  *M = DenseMeta{dq.trim ? e->d_trim_vocab.as<uint32_t>() : nullptr, e->has_added ? e->d_trim_added.as<AddedTrim>() : nullptr,
+                 e->has_added ? e->n_trim_added : 0u, dq.aps ? 1u : 0u, dq.word_ids ? ws.word_ids.as<uint32_t>() : nullptr,
+                 dq.special_mask ? ws.dense_special.as<uint8_t>() : nullptr, dq.seq_ids ? ws.dense_seq.as<int8_t>() : nullptr,
+                 dq.word_ids ? ws.dense_word.as<uint32_t>() : nullptr, &ws.ctl.as<ctl_block>()->err};
+  return B2T_OK;
 }
 
 // CSR of the workspace -> dense rows in ws.dense_* (asynchronous on st).  n_inputs = documents / docs_per_row; n_rows =
@@ -550,8 +591,12 @@ static int launch_dense(b2t_engine* e, Workspace& ws, uint32_t n_inputs, uint32_
     DenseOverflow O{ws.row_sample.as<uint32_t>(), ws.row_base.as<uint32_t>(), sample_base, dq.stride,
                     b_first ? dq.type_ob : dq.type_oa, b_first ? dq.type_oa : dq.type_ob,
                     dq.offsets ? ws.offsets.as<uint2>() : nullptr, dq.offsets ? ws.dense_off.as<uint2>() : nullptr};
+    DenseMeta M{};
+    if (dq.meta() && (rc = make_meta(e, ws, cells, dq, &M))) return rc;
     if (n_rows && dq.L()) {
-      if (dq.offsets) launch_rows<true, true>(ws, n_rows, dq, O, st);
+      if (dq.meta() && dq.offsets) launch_rows<true, true, true>(ws, n_rows, dq, O, st, M);
+      else if (dq.meta()) launch_rows<true, false, true>(ws, n_rows, dq, O, st, M);
+      else if (dq.offsets) launch_rows<true, true>(ws, n_rows, dq, O, st);
       else launch_rows<true, false>(ws, n_rows, dq, O, st);
     }
     e->last_launches++;
@@ -559,10 +604,17 @@ static int launch_dense(b2t_engine* e, Workspace& ws, uint32_t n_inputs, uint32_
     CU(cudaGetLastError());
     return B2T_OK;
   }
-  if (dq.offsets) {   // offset rows of the kept parts only: the <0, 1> instantiations
-    if ((rc = ws.dense_off.ensure(cells * 8 + 16))) return rc;
-    const DenseOverflow O{nullptr, nullptr, 0u, 0u, 0u, 0u, ws.offsets.as<uint2>(), ws.dense_off.as<uint2>()};
-    if (n_rows && dq.L()) launch_rows<false, true>(ws, n_rows, dq, O, st);
+  if (dq.offsets || dq.meta()) {   // offset rows of the kept parts only (the <0, 1> instantiations) and / or row metadata (<0, *, 1>)
+    if (dq.offsets && (rc = ws.dense_off.ensure(cells * 8 + 16))) return rc;
+    DenseOverflow O{};
+    if (dq.offsets) O = DenseOverflow{nullptr, nullptr, 0u, 0u, 0u, 0u, ws.offsets.as<uint2>(), ws.dense_off.as<uint2>()};
+    DenseMeta M{};
+    if (dq.meta() && (rc = make_meta(e, ws, cells, dq, &M))) return rc;
+    if (n_rows && dq.L()) {
+      if (dq.meta() && dq.offsets) launch_rows<false, true, true>(ws, n_rows, dq, O, st, M);
+      else if (dq.meta()) launch_rows<false, false, true>(ws, n_rows, dq, O, st, M);
+      else launch_rows<false, true>(ws, n_rows, dq, O, st);
+    }
     e->last_launches++;
     CU(cudaGetLastError());
     return B2T_OK;
@@ -884,6 +936,22 @@ static int run_device_pipeline(b2t_engine* e, Workspace& ws, cudaStream_t st) {
   return B2T_OK;
 }
 
+static int trim_ambiguous() {
+  return fail(B2T_ERR_UNSUPPORTED, "offset trimming: an added token with both lstrip and rstrip absorbed whitespace, and its offsets do not tell "
+              "on which side; trim_offsets is not available for this batch");
+}
+
+// Row kernels that run after the host has read the control block (overflowing parts, BatchLongest): an offset trimming
+// that may meet an lstrip + rstrip added token reads the control block's error word again once they are done.
+static int meta_check(b2t_engine* e, Workspace& ws, const DenseReq& dq, cudaStream_t st) {
+  if (!dq.trim || !e->has_added || !e->added_both) return B2T_OK;
+  ctl_block* h = ws.h_ctl.as<ctl_block>();
+  CU(cudaMemcpyAsync(&h->err, &ws.ctl.as<ctl_block>()->err, 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (h->err & ERR_INTERNAL) return fail(B2T_ERR_CUDA, "internal error: a marked added-token id without an added token");
+  return (h->err & ERR_TRIM_AMBIGUOUS) ? trim_ambiguous() : B2T_OK;
+}
+
 // Checks the control block of a run the host has waited for.  While the long pool was too small (rare: the batch holds
 // more bytes of long pre-tokens than the pool), grows it to what the run asked for and repeats ws.req on st, three runs
 // in all.  *reran tells whether the run was repeated.
@@ -899,6 +967,7 @@ static int check_run(b2t_engine* e, Workspace& ws, cudaStream_t st, bool* reran 
       if (c->err & ERR_STRIDE)
         return fail(B2T_ERR_TRUNCATION, "`stride` must be strictly less than `max_len=%u` (note that `max_len` may be shorter than the max length of the "
                     "original model, as it subtracts the number of special characters", c->stride_m);
+      if (c->err & ERR_TRIM_AMBIGUOUS) return trim_ambiguous();
       return B2T_OK;
     }
     if (attempt >= 2) return fail(B2T_ERR_CUDA, "long pool did not converge");
@@ -951,7 +1020,7 @@ static int device_encode(const char* fn, b2t_engine* e, const void* out, const u
   if (((uintptr_t)d_bytes & 15u) != 0) return fail(B2T_ERR_INVALID, "%s: d_bytes must be 16-byte aligned", fn);
   int rc;
   if (dq && (rc = make_dense_req(spec, dq))) return rc;
-  if (dq && dq->offsets) flags |= B2T_WANT_OFFSETS;   // offset rows come from the CSR's offsets
+  if (dq && (rc = dense_engine_flags(e, *dq, &flags))) return rc;   // offset rows come from the CSR's offsets, word ids from its word ids
   std::lock_guard<std::mutex> lk(e->dev_mu);
   CU(cudaSetDevice(e->device));
   cudaStream_t st = stream ? (cudaStream_t)stream : e->own_stream;
@@ -1010,7 +1079,7 @@ extern "C" int b2t_engine_set_added_tokens(b2t_engine* e, uint32_t n_tokens, con
   if (!e) return fail(B2T_ERR_INVALID, "null engine");
   std::lock_guard<std::mutex> lk(e->dev_mu);
   CU(cudaSetDevice(e->device));
-  e->has_added = 0;
+  e->has_added = 0; e->added_both = 0; e->n_trim_added = 0;
   if (n_tokens == 0) return B2T_OK;
   if (!bytes || !off || !ids || !flags) return fail(B2T_ERR_INVALID, "b2t_engine_set_added_tokens: null argument");
   if (e->add_prefix_space) return fail(B2T_ERR_UNSUPPORTED, "added-token extraction on the device does not combine with add_prefix_space");
@@ -1064,6 +1133,21 @@ extern "C" int b2t_engine_set_added_tokens(b2t_engine* e, uint32_t n_tokens, con
     for (uint32_t b = 0; b < 256; ++b) if (((first[b >> 5] | first[8 + (b >> 5)]) >> (b & 31)) & 1u) fb.push_back(b);
     if (fb.size() <= 4) { e->at.n_first = (uint32_t)fb.size(); for (size_t i = 0; i < fb.size(); ++i) e->at.first_bcast[i] = fb[i] * 0x01010101u; }
   }
+  // offset trimming in dense rows: per token, by ascending id, its char count and leading / trailing whitespace-or-U+0120
+  // counts, all-whitespace and its lstrip / rstrip flags (dense_kernels.cuh added_trim_counts)
+  std::vector<AddedTrim> trim;
+  for (int s2 = 0; s2 < 2; ++s2)
+    for (uint32_t i : order[s2]) {
+      uint32_t chars, lead, trail;
+      space_counts(bytes + off[i], off[i + 1] - off[i], cls.data(), &chars, &lead, &trail);
+      const bool l = (flags[i] & B2T_ADDED_LSTRIP) != 0, r = (flags[i] & B2T_ADDED_RSTRIP) != 0;
+      trim.push_back(AddedTrim{ids[i], chars, std::min(lead, 0xFFFFu) | std::min(trail, 0xFFFFu) << 16,
+                               (lead == chars ? TRIM_ALL_SPACE : 0u) | (l ? TRIM_LSTRIP : 0u) | (r ? TRIM_RSTRIP : 0u)});
+      if (l && r) e->added_both = 1;
+    }
+  std::stable_sort(trim.begin(), trim.end(), [](const AddedTrim& a, const AddedTrim& b) { return a.id < b.id; });
+  if ((rc = upload(e->d_trim_added, trim))) return rc;
+  e->n_trim_added = (uint32_t)trim.size();
   e->has_added = 1;
   return B2T_OK;
 }
@@ -1099,7 +1183,7 @@ static int dense_device(const char* fn, b2t_engine* e, const uint8_t* d_bytes, u
       return fail(B2T_ERR_INVALID, "a row of %u tokens does not fit the dense length %u: enable truncation (the reference returns a longer row here)", max_row, dq.L());
     if (dq.overflow && (rc2 = overflow_rows(c, 0, dq.L(), &n_rows))) return rc2;
     // asynchronous on st, like the CSR entry point's result (a fixed length without overflowing parts: queued already)
-    if ((dq.batch_longest || dq.overflow) && (rc2 = launch_dense(e, ws, n_in, n_rows, dq, st))) return rc2;
+    if ((dq.batch_longest || dq.overflow) && ((rc2 = launch_dense(e, ws, n_in, n_rows, dq, st)) || (rc2 = meta_check(e, ws, dq, st)))) return rc2;
     b2t_result* r = new b2t_result();
     r->eng = e; r->on_device = 1; r->n_docs = n_in; r->n_rows = n_rows;
     r->row_sample = dq.overflow ? ws.row_sample.as<uint32_t>() : nullptr;
@@ -1109,6 +1193,9 @@ static int dense_device(const char* fn, b2t_engine* e, const uint8_t* d_bytes, u
     r->dense_ids = ws.dense_ids.as<uint32_t>(); r->row_len = ws.dense_len.as<uint32_t>();
     r->dense_mask = dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr;
     r->type_ids = dq.pairs() ? ws.dense_type.as<uint8_t>() : nullptr;
+    r->special_mask = dq.special_mask ? ws.dense_special.as<uint8_t>() : nullptr;
+    r->seq_ids = dq.seq_ids ? ws.dense_seq.as<int8_t>() : nullptr;
+    r->dense_word = dq.word_ids ? ws.dense_word.as<uint32_t>() : nullptr;
     *out = r;
     return B2T_OK;
   });
@@ -1140,6 +1227,7 @@ static b2t_result* pool_get(b2t_engine* e) {
   if (!e->pool.empty()) {
     b2t_result* r = e->pool.back().release(); e->pool.pop_back();
     r->type_ids = nullptr; r->n_rows = 0; r->row_sample = nullptr; r->dense_off = nullptr;
+    r->special_mask = nullptr; r->seq_ids = nullptr; r->dense_word = nullptr;
     return r;
   }
   return new b2t_result();
@@ -1191,6 +1279,9 @@ static int queue_dense_copy(b2t_result* r, const Workspace& ws, uint32_t r0, uin
     if (dq.want_mask) CU(cudaMemcpyAsync(r->h_dense_mask.as<uint8_t>() + (size_t)r0 * L, ws.dense_mask.p, (size_t)nr * L, cudaMemcpyDeviceToHost, ws.stream));
     if (dq.pairs()) CU(cudaMemcpyAsync(r->h_type_ids.as<uint8_t>() + (size_t)r0 * L, ws.dense_type.p, (size_t)nr * L, cudaMemcpyDeviceToHost, ws.stream));
     if (dq.offsets) CU(cudaMemcpyAsync(r->h_dense_off.as<uint32_t>() + (size_t)r0 * L * 2, ws.dense_off.p, (size_t)nr * L * 8, cudaMemcpyDeviceToHost, ws.stream));
+    if (dq.special_mask) CU(cudaMemcpyAsync(r->h_special.as<uint8_t>() + (size_t)r0 * L, ws.dense_special.p, (size_t)nr * L, cudaMemcpyDeviceToHost, ws.stream));
+    if (dq.seq_ids) CU(cudaMemcpyAsync(r->h_seq.as<int8_t>() + (size_t)r0 * L, ws.dense_seq.p, (size_t)nr * L, cudaMemcpyDeviceToHost, ws.stream));
+    if (dq.word_ids) CU(cudaMemcpyAsync(r->h_word.as<uint32_t>() + (size_t)r0 * L, ws.dense_word.p, (size_t)nr * L * 4, cudaMemcpyDeviceToHost, ws.stream));
   }
   if (nr) CU(cudaMemcpyAsync(r->h_row_len.as<uint32_t>() + r0, ws.dense_len.p, (size_t)nr * 4, cudaMemcpyDeviceToHost, ws.stream));
   if (nr && dq.overflow) CU(cudaMemcpyAsync(r->h_row_sample.as<uint32_t>() + r0, ws.row_sample.p, (size_t)nr * 4, cudaMemcpyDeviceToHost, ws.stream));
@@ -1198,14 +1289,14 @@ static int queue_dense_copy(b2t_result* r, const Workspace& ws, uint32_t r0, uin
 }
 
 static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, uint32_t flags,
-                       b2t_result** out, const DenseReq* dq_in = nullptr) {
+                       b2t_result** out, const DenseReq* dq_in = nullptr, uint32_t dq_flags = 0u) {
   const uint64_t total_bytes = doc_off[n_docs];
   // ---- split into chunks of whole documents
   std::vector<Chunk> chunks;
   uint64_t max_chunk = 0;
   DenseReq dq_local;
   DenseReq* dq = nullptr;
-  if (dq_in) { dq_local = *dq_in; dq = &dq_local; flags = dq->offsets ? B2T_WANT_OFFSETS : 0u; }   // (offset rows: from the CSR's offsets)
+  if (dq_in) { dq_local = *dq_in; dq = &dq_local; flags = dq_flags; }   // (offset rows, word ids: from the CSR's)
   // BatchLongest padding needs every row length before the first row can be written: the batch runs as one chunk
   if (dq && dq->batch_longest && total_bytes + n_docs >= (1ull << 31))
     return fail(B2T_ERR_UNSUPPORTED, "dense output padded to the longest row needs the batch in one device pass (< 2^31 bytes); pad to a fixed length instead");
@@ -1241,6 +1332,7 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     return B2T_OK;
   };
   r->dense_len = 0; r->dense_ids = nullptr; r->dense_mask = nullptr; r->row_len = nullptr; r->type_ids = nullptr;
+  r->special_mask = nullptr; r->seq_ids = nullptr; r->dense_word = nullptr;
   // pinned rows: the whole batch's n_rows rows, or with overflowing parts a guess grown on demand (contents kept)
   uint64_t cap_rows = 0, row_total = 0;
   auto dense_host = [&](uint32_t L, uint64_t rows, bool keep) -> int {
@@ -1248,7 +1340,9 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     const size_t cells = (size_t)rows * L;
     if ((rc2 = r->h_dense_ids.ensure(cells * 4 + 16, keep)) || (rc2 = r->h_row_len.ensure((size_t)rows * 4 + 16, keep)) ||
         (dq->want_mask && (rc2 = r->h_dense_mask.ensure(cells + 16, keep))) || (dq->pairs() && (rc2 = r->h_type_ids.ensure(cells + 16, keep))) ||
-        (dq->overflow && (rc2 = r->h_row_sample.ensure((size_t)rows * 4 + 16, keep))) || (dq->offsets && (rc2 = r->h_dense_off.ensure(cells * 8 + 16, keep))))
+        (dq->overflow && (rc2 = r->h_row_sample.ensure((size_t)rows * 4 + 16, keep))) || (dq->offsets && (rc2 = r->h_dense_off.ensure(cells * 8 + 16, keep))) ||
+        (dq->special_mask && (rc2 = r->h_special.ensure(cells + 16, keep))) || (dq->seq_ids && (rc2 = r->h_seq.ensure(cells + 16, keep))) ||
+        (dq->word_ids && (rc2 = r->h_word.ensure(cells * 4 + 16, keep))))
       return rc2;
     cap_rows = rows;
     return B2T_OK;
@@ -1289,7 +1383,8 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
           if ((rc2 = dense_host(dq->L(), std::max<uint64_t>((row_total + nr) * 2, (uint64_t)n_rows), true))) return rc2;
         }
       }
-      if ((dq->batch_longest || dq->overflow) && (rc2 = launch_dense(e, ws, n_in, nr, *dq, ws.stream, c.d0 / per))) return rc2;
+      if ((dq->batch_longest || dq->overflow) && ((rc2 = launch_dense(e, ws, n_in, nr, *dq, ws.stream, c.d0 / per)) || (rc2 = meta_check(e, ws, *dq, ws.stream))))
+        return rc2;
       // (a fixed length without overflowing parts: the rows were queued for the copy right behind the kernels, see issue();
       // a rerun has replaced them)
       if ((dq->batch_longest || dq->overflow || reran) && (rc2 = queue_dense_copy(r, ws, (uint32_t)row_total, nr, *dq))) return rc2;
@@ -1360,6 +1455,9 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     r->n_rows = (uint32_t)row_total;
     r->row_sample = dq->overflow ? r->h_row_sample.as<uint32_t>() : nullptr;
     r->dense_off = dq->offsets ? r->h_dense_off.as<uint32_t>() : nullptr;
+    r->special_mask = dq->special_mask ? r->h_special.as<uint8_t>() : nullptr;
+    r->seq_ids = dq->seq_ids ? r->h_seq.as<int8_t>() : nullptr;
+    r->dense_word = dq->word_ids ? r->h_word.as<uint32_t>() : nullptr;
   } else {
     // chunk-relative row_ptr -> batch-relative (host fix-up: one addition per document)
     uint64_t* rp = r->h_row_ptr.as<uint64_t>();
@@ -1385,7 +1483,9 @@ static int host_call(const char* fn, b2t_engine* e, const uint8_t* bytes, const 
                      const Spec* spec, DenseReq* dq, Run&& run) {
   if (!e || !out || !doc_off || (!bytes && doc_off[n_docs])) return fail(B2T_ERR_INVALID, "%s: null argument", fn);
   int rc;
+  uint32_t dq_flags = 0;
   if (dq && (rc = make_dense_req(spec, dq))) return rc;
+  if (dq && (rc = dense_engine_flags(e, *dq, &dq_flags))) return rc;
   if (doc_off[0] != 0) return fail(B2T_ERR_INVALID, "doc_off[0] must be 0");
   for (uint32_t d = 0; d < n_docs; ++d)  // the kernels index the buffer with these: a decreasing offset must never reach them
     if (doc_off[d + 1] < doc_off[d]) return fail(B2T_ERR_INVALID, "doc_off must be non-decreasing (document %u)", d);
@@ -1393,20 +1493,20 @@ static int host_call(const char* fn, b2t_engine* e, const uint8_t* bytes, const 
   SetLease lease(e);
   if (e->profiling) prof.lock();
   CU(cudaSetDevice(e->device));
-  return run(*lease.ss);
+  return run(*lease.ss, dq_flags);
 }
 
 extern "C" int b2t_encode_batch(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, uint32_t flags,
                                 b2t_result** out) {
   return host_call("b2t_encode_batch", e, bytes, doc_off, n_docs, out, NO_SPEC, nullptr,
-                   [&](b2t_engine::SlotSet& ss) { return host_encode(e, ss, bytes, doc_off, n_docs, flags, out); });
+                   [&](b2t_engine::SlotSet& ss, uint32_t) { return host_encode(e, ss, bytes, doc_off, n_docs, flags, out); });
 }
 
 extern "C" int b2t_encode_batch_dense(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, const b2t_dense_spec* spec,
                                       b2t_result** out) {
   DenseReq dq;
   return host_call("b2t_encode_batch_dense", e, bytes, doc_off, n_docs, out, spec, &dq,
-                   [&](b2t_engine::SlotSet& ss) { return host_encode(e, ss, bytes, doc_off, n_docs, 0u, out, &dq); });
+                   [&](b2t_engine::SlotSet& ss, uint32_t dq_flags) { return host_encode(e, ss, bytes, doc_off, n_docs, 0u, out, &dq, dq_flags); });
 }
 
 // Replaces TokenizerImpl::post_process for a batch of pairs (tokenizer/mod.rs:1265-1317), see include/b2t.h
@@ -1417,7 +1517,7 @@ extern "C" int b2t_encode_pairs_dense(b2t_engine* e, const uint8_t* bytes, const
   int rc = pair_docs("b2t_encode_pairs_dense", n_pairs, &n_docs);
   if (rc) return rc;
   return host_call("b2t_encode_pairs_dense", e, bytes, doc_off, n_docs, out, spec, &dq,
-                   [&](b2t_engine::SlotSet& ss) { return host_encode(e, ss, bytes, doc_off, n_docs, 0u, out, &dq); });
+                   [&](b2t_engine::SlotSet& ss, uint32_t dq_flags) { return host_encode(e, ss, bytes, doc_off, n_docs, 0u, out, &dq, dq_flags); });
 }
 
 // PreTokenizer seam: runs K0/K1 and expands the split bitmaps into (start, end) pairs.  The expansion of the bitmap
@@ -1475,7 +1575,7 @@ static int pre_tokenize(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* b
 
 extern "C" int b2t_pre_tokenize_batch(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, b2t_result** out) {
   return host_call("b2t_pre_tokenize_batch", e, bytes, doc_off, n_docs, out, NO_SPEC, nullptr,
-                   [&](b2t_engine::SlotSet& ss) { return pre_tokenize(e, ss, bytes, doc_off, n_docs, out); });
+                   [&](b2t_engine::SlotSet& ss, uint32_t) { return pre_tokenize(e, ss, bytes, doc_off, n_docs, out); });
 }
 
 // ------------------------------------------------------------------------------------------------ results
@@ -1494,6 +1594,9 @@ extern "C" const uint8_t* b2t_result_type_ids(const b2t_result* r) { return r ? 
 extern "C" uint32_t b2t_result_dense_rows(const b2t_result* r) { return r ? r->n_rows : 0; }
 extern "C" const uint32_t* b2t_result_row_sample(const b2t_result* r) { return r ? r->row_sample : nullptr; }
 extern "C" const uint32_t* b2t_result_dense_offsets(const b2t_result* r) { return r ? r->dense_off : nullptr; }
+extern "C" const uint8_t* b2t_result_special_tokens_mask(const b2t_result* r) { return r ? r->special_mask : nullptr; }
+extern "C" const int8_t* b2t_result_sequence_ids(const b2t_result* r) { return r ? r->seq_ids : nullptr; }
+extern "C" const uint32_t* b2t_result_dense_word_ids(const b2t_result* r) { return r ? r->dense_word : nullptr; }
 extern "C" void b2t_result_free(b2t_result* r) {
   if (!r) return;
   if (r->on_device || !r->eng) { delete r; return; }

@@ -4,6 +4,8 @@
 #include <string.h>
 #include <vector_types.h>
 
+#include <algorithm>
+
 #include "pretok_logic.cuh"
 #include "unicode_ranges.inc"
 #include "bert_tables.inc"
@@ -29,6 +31,37 @@ void unicode_class_table(int scheme, uint8_t* out) {
     fill(B2T_RUST_W, B2T_RUST_W_COUNT, CLS_L);
     fill(B2T_RUST_S, B2T_RUST_S_COUNT, CLS_S);
   }
+}
+
+void space_counts(const uint8_t* s, uint32_t len, const uint8_t* cls, uint32_t* chars, uint32_t* lead, uint32_t* trail) {
+  std::vector<bool> sp;
+  for (uint32_t i = 0; i < len;) {   // (a malformed sequence counts as one char per byte, not as whitespace)
+    const uint8_t b = s[i];
+    uint32_t n = b < 0x80 ? 1 : (b >> 5) == 6 ? 2 : (b >> 4) == 14 ? 3 : (b >> 3) == 30 ? 4 : 1;
+    if (i + n > len) n = 1;
+    uint32_t cp = n == 1 ? b : (uint32_t)(b & (0x7F >> n));
+    for (uint32_t k = 1; k < n; ++k) cp = (cp << 6) | (s[i + k] & 63u);
+    sp.push_back(cp == 0x120u || (cp < 0x110000 && cls[cp] == CLS_S && (n > 1 || b < 0x80)));
+    i += n;
+  }
+  uint32_t l = 0, t = 0;
+  while (l < sp.size() && sp[l]) ++l;
+  while (t < sp.size() && sp[sp.size() - 1 - t]) ++t;
+  *chars = (uint32_t)sp.size(); *lead = l; *trail = t;
+}
+
+std::vector<uint32_t> vocab_trim_counts(uint32_t n_vocab, const uint8_t* vocab_bytes, const uint32_t* vocab_off, const uint32_t* vocab_ids) {
+  uint32_t n_ids = 0;
+  for (uint32_t i = 0; i < n_vocab; ++i) n_ids = std::max(n_ids, vocab_ids[i] + 1);
+  std::vector<uint8_t> cls(0x110000);
+  unicode_class_table(1, cls.data());
+  std::vector<uint32_t> out(n_ids, 0u);
+  for (uint32_t i = 0; i < n_vocab; ++i) {
+    uint32_t chars, lead, trail;
+    space_counts(vocab_bytes + vocab_off[i], vocab_off[i + 1] - vocab_off[i], cls.data(), &chars, &lead, &trail);
+    out[vocab_ids[i]] = std::min(lead, 0xFFFFu) | std::min(trail, 0xFFFFu) << 16;
+  }
+  return out;
 }
 
 static void utf8_append(std::string& s, uint32_t cp);

@@ -43,6 +43,13 @@ void build_bert_norm(bool clean_text, bool handle_chinese_chars, bool strip_acce
 // 2 = BertPreTokenizer: CLS_S whitespace, CLS_O punctuation, CLS_L everything else).
 void unicode_class_table(int scheme, uint8_t* out);
 
+// A token string as ByteLevel::process_offsets (pre_tokenizers/byte_level.rs:202-234) counts it: its chars, and its
+// leading / trailing chars that are U+0120 or whitespace (cls: scheme 1 of unicode_class_table, \s = CLS_S).
+void space_counts(const uint8_t* s, uint32_t len, const uint8_t* cls, uint32_t* chars, uint32_t* lead, uint32_t* trail);
+
+// Per vocabulary id (ids above the largest are not in the table): space_counts' lead | trail << 16 of its string.
+std::vector<uint32_t> vocab_trim_counts(uint32_t n_vocab, const uint8_t* vocab_bytes, const uint32_t* vocab_off, const uint32_t* vocab_ids);
+
 // Returns "" on success, else an error message; *vocab_err distinguishes B2T_ERR_VOCAB from B2T_ERR_UNSUPPORTED.
 std::string build_host_tables(int model, int pretok, int ignore_merges, uint32_t n_vocab, const uint8_t* vocab_bytes,
                               const uint32_t* vocab_off, const uint32_t* vocab_ids, uint32_t n_merges,

@@ -813,9 +813,11 @@ class Tokenizer:
         return out
 
     # ---- dense mode: template + truncation + padding on the device (include/b2t.h b2t_encode_batch_dense, b2t_encode_pairs_dense)
-    def _dense_fields(self, sp, want_mask, overflow=False, offsets=False):
+    def _dense_fields(self, sp, want_mask, overflow=False, offsets=False, trim_offsets=False, special_mask=False, sequence_ids=False,
+                      word_ids=False):
         """the padding / truncation fields b2t_dense_spec and b2t_pair_dense_spec share, filled into sp; overflow / offsets:
-        return_overflowing_tokens / return_offsets_mapping"""
+        return_overflowing_tokens / return_offsets_mapping; trim_offsets: offset rows as the post-processor leaves them
+        (trimmed where it trims); special_mask / sequence_ids / word_ids: the row metadata"""
         tr, pd = self._truncation, self._padding
         if pd is None:
             raise UnsupportedConfig("dense output needs padding enabled (enable_padding): rows must share one length")
@@ -829,24 +831,36 @@ class Tokenizer:
         sp.truncate_left = int(tr is not None and tr["direction"] == "left")
         sp.pad_left = int(pd["direction"] == "left")
         sp.want_mask = int(want_mask)
-        if offsets and self._template is not None and self._template["trim"] is not None:
-            raise UnsupportedConfig("offsets behind a post-processor that trims them (trim_offsets) have no dense form")
+        trims = self._template is not None and self._template["trim"] is not None
+        if offsets and trims and not trim_offsets:
+            raise UnsupportedConfig("offsets behind a post-processor that trims them (trim_offsets) have no dense form without trim_offsets=True")
         sp.stride = int(tr["stride"]) if (overflow and tr is not None) else 0
         sp.dense_flags = (_lib.DENSE_OVERFLOW if overflow else 0) | (_lib.DENSE_OFFSETS if offsets else 0)
+        if offsets and trims:
+            sp.dense_flags |= _lib.DENSE_TRIM_OFFSETS | (_lib.DENSE_TRIM_PREFIX_SPACE if self._template["trim"] else 0)
+        if sequence_ids and self._template is None:
+            # without a post-processor the reference's default_process keeps sequence ranges on the kept parts only, and a
+            # sequence without ranges reads as sequence 0 over its whole length, padding included
+            raise UnsupportedConfig("sequence ids of a tokenizer without a post-processor have no dense form")
+        sp.dense_flags |= ((_lib.DENSE_SPECIAL_MASK if special_mask else 0) | (_lib.DENSE_SEQUENCE_IDS if sequence_ids else 0) |
+                           (_lib.DENSE_WORD_IDS if word_ids else 0))
         return sp
 
-    def dense_spec(self, add_special_tokens=True, want_mask=True, return_overflowing_tokens=False, return_offsets_mapping=False):
+    def dense_spec(self, add_special_tokens=True, want_mask=True, return_overflowing_tokens=False, return_offsets_mapping=False,
+                   trim_offsets=False, return_special_tokens_mask=False, return_sequence_ids=False, return_word_ids=False):
         """The tokenizer's truncation / padding / single-sequence template as a b2t_dense_spec (+ the arrays it points to)."""
         tp = self._template
         pre = [t for t, _ in tp["pre"]] if (tp is not None and add_special_tokens) else []
         post = [t for t, _ in tp["post"]] if (tp is not None and add_special_tokens) else []
-        sp = self._dense_fields(_lib.DenseSpec(), want_mask, return_overflowing_tokens, return_offsets_mapping)
+        sp = self._dense_fields(_lib.DenseSpec(), want_mask, return_overflowing_tokens, return_offsets_mapping, trim_offsets,
+                                return_special_tokens_mask, return_sequence_ids, return_word_ids)
         keep = (np.asarray(pre, dtype=np.uint32), np.asarray(post, dtype=np.uint32))
         sp.n_pre, sp.n_post = len(pre), len(post)
         sp.pre_ids, sp.post_ids = (keep[0].ctypes.data if pre else None), (keep[1].ctypes.data if post else None)
         return sp, keep
 
-    def pair_dense_spec(self, add_special_tokens=True, want_mask=True, return_overflowing_tokens=False, return_offsets_mapping=False):
+    def pair_dense_spec(self, add_special_tokens=True, want_mask=True, return_overflowing_tokens=False, return_offsets_mapping=False,
+                        trim_offsets=False, return_special_tokens_mask=False, return_sequence_ids=False, return_word_ids=False):
         """The tokenizer's truncation / padding / pair template as a b2t_pair_dense_spec (+ the arrays it points to).  The
         pieces come from the template's pair form (default_process without a post-processor: A type 0, B type 1); without
         special tokens the two sequence pieces stay, in their order and with their type ids (processors/template.rs:554-560).
@@ -855,7 +869,8 @@ class Tokenizer:
         pieces = [("seq", 0, 0), ("seq", 1, 1)] if tp is None else tp["pair"]
         if pieces is None:
             raise ValueError("the post-processor has no template for pairs of sequences")
-        sp = self._dense_fields(_lib.PairDenseSpec(), want_mask, return_overflowing_tokens, return_offsets_mapping)
+        sp = self._dense_fields(_lib.PairDenseSpec(), want_mask, return_overflowing_tokens, return_offsets_mapping, trim_offsets,
+                                return_special_tokens_mask, return_sequence_ids, return_word_ids)
         pieces = [p for p in pieces if p[0] == "seq" or add_special_tokens]
         ot = tp.get("overflow_type") if (tp is not None and add_special_tokens) else None   # (pairs.post_process's rule)
         sp.overflow_type_a, sp.overflow_type_b = (0, 1) if ot is None else (ot, ot)
@@ -873,7 +888,8 @@ class Tokenizer:
 
     def _dense_call(self, entry, data, doc_off, n_rows, sp, want_mask, type_ids):
         """b2t_encode_batch_dense / b2t_encode_pairs_dense -> (ids [R, L], mask [R, L] | None, lengths [R], type ids [R, L] | None,
-        row sample [R] | None, offsets [R, L, 2] | None); R = n_rows without overflowing parts"""
+        row sample [R] | None, offsets [R, L, 2] | None, special-tokens mask [R, L] | None, sequence ids [R, L] | None, word ids
+        [R, L] | None); R = n_rows without overflowing parts"""
         if self._added is not None and not self._dev_added and added.split_batch(self._added, data, doc_off)[2]:
             raise UnsupportedConfig("the batch contains added tokens and this configuration extracts them on the host: use encode_batch")
         L = _lib.lib()
@@ -887,20 +903,31 @@ class Tokenizer:
                     _view(L.b2t_result_row_lengths(res), R, np.uint32),
                     _view(L.b2t_result_type_ids(res), R * W, np.uint8).reshape(R, W) if type_ids else None,
                     _view(L.b2t_result_row_sample(res), R, np.uint32) if sp.dense_flags & _lib.DENSE_OVERFLOW else None,
-                    _view(L.b2t_result_dense_offsets(res), 2 * R * W, np.uint32).reshape(R, W, 2) if sp.dense_flags & _lib.DENSE_OFFSETS else None)
+                    _view(L.b2t_result_dense_offsets(res), 2 * R * W, np.uint32).reshape(R, W, 2) if sp.dense_flags & _lib.DENSE_OFFSETS else None,
+                    _view(L.b2t_result_special_tokens_mask(res), R * W, np.uint8).reshape(R, W) if sp.dense_flags & _lib.DENSE_SPECIAL_MASK else None,
+                    _view(L.b2t_result_sequence_ids(res), R * W, np.int8).reshape(R, W) if sp.dense_flags & _lib.DENSE_SEQUENCE_IDS else None,
+                    _view(L.b2t_result_dense_word_ids(res), R * W, np.uint32).reshape(R, W) if sp.dense_flags & _lib.DENSE_WORD_IDS else None)
         return _read_result(self, res, views)[0]
 
     @staticmethod
     def _dense_dict(out, rows, overflow, offsets):
-        """the dict of a dense call: rows = what _dense_call returned, plus the optional overflow / offset entries"""
+        """the dict of a dense call: rows = what _dense_call returned, plus the optional overflow / offset / metadata entries
+        (word ids as int32 with -1 for None)"""
         if overflow:
             out["overflow_to_sample_mapping"] = rows[4]
         if offsets:
             out["offset_mapping"] = rows[5]
+        if rows[6] is not None:
+            out["special_tokens_mask"] = rows[6]
+        if rows[7] is not None:
+            out["sequence_ids"] = rows[7]
+        if rows[8] is not None:
+            out["word_ids"] = rows[8].view(np.int32)
         return out
 
     def encode_batch_dense(self, data, doc_off=None, add_special_tokens=True, want_mask=True, return_overflowing_tokens=False,
-                           return_offsets_mapping=False):
+                           return_offsets_mapping=False, trim_offsets=False, return_special_tokens_mask=False, return_sequence_ids=False,
+                           return_word_ids=False):
         """Batch of single sequences -> {"input_ids": uint32[n, L], "attention_mask": uint8[n, L] | None, "lengths": uint32[n]}
         with the tokenizer's truncation, template and padding applied on the device (what `encode_batch` + stacking the
         Encodings' ids / attention_mask gives in the reference).  `data` is a list of str, or packed (np.uint8[N], np.uint64[n+1]).
@@ -908,23 +935,33 @@ class Tokenizer:
         too -- each input's kept row, then its overflowing rows, what stacking `[e] + e.overflowing` gives -- and the dict
         gains "overflow_to_sample_mapping" (uint32[R], the input of each row).  return_offsets_mapping: "offset_mapping"
         (uint32[R, L, 2], char offsets; (0, 0) for special tokens and padding).  An overflowing row longer than L is refused
-        (B2TError; the reference returns it longer and unpadded); a stride not below a sequence's max_len raises ValueError."""
+        (B2TError; the reference returns it longer and unpadded); a stride not below a sequence's max_len raises ValueError.
+        trim_offsets: the offset rows as the post-processor leaves them -- trimmed (ByteLevel process_offsets, every part on its
+        own) where it trims offsets, unchanged where it does not; without it offsets behind a trimming post-processor raise
+        UnsupportedConfig.  An added token with both lstrip and rstrip that absorbed whitespace raises UnsupportedConfig there.
+        return_special_tokens_mask / return_sequence_ids / return_word_ids: "special_tokens_mask" (uint8[R, L], 1 for template
+        tokens and padding), "sequence_ids" (int8[R, L], -1 = None) and "word_ids" (int32[R, L], -1 = None), as the reference's
+        Encoding has them."""
         if doc_off is None:
             data, doc_off = _pack(data, np.uint64)
         data = np.ascontiguousarray(data, dtype=np.uint8)
         doc_off = np.ascontiguousarray(doc_off, dtype=np.uint64)
-        sp, keep = self.dense_spec(add_special_tokens, want_mask, return_overflowing_tokens, return_offsets_mapping)
+        sp, keep = self.dense_spec(add_special_tokens, want_mask, return_overflowing_tokens, return_offsets_mapping, trim_offsets,
+                                   return_special_tokens_mask, return_sequence_ids, return_word_ids)
         try:
             rows = self._dense_call("b2t_encode_batch_dense", data, doc_off, len(doc_off) - 1, sp, want_mask, False)
         except B2TError as ex:
             if ex.code == _lib.B2T_ERR_TRUNCATION:   # the reference's stride panic, with its message
                 raise ValueError(str(ex)) from None
+            if ex.code == _lib.B2T_ERR_UNSUPPORTED and sp.dense_flags & _lib.DENSE_TRIM_OFFSETS:   # (the lstrip + rstrip refusal)
+                raise UnsupportedConfig(str(ex)) from None
             raise
         return self._dense_dict({"input_ids": rows[0], "attention_mask": rows[1], "lengths": rows[2]}, rows, return_overflowing_tokens,
                                 return_offsets_mapping)
 
     def encode_pairs_dense(self, pairs, doc_off=None, add_special_tokens=True, want_mask=True, return_overflowing_tokens=False,
-                           return_offsets_mapping=False):
+                           return_offsets_mapping=False, trim_offsets=False, return_special_tokens_mask=False, return_sequence_ids=False,
+                           return_word_ids=False):
         """Batch of pairs of sequences -> {"input_ids": uint32[n, L], "token_type_ids": uint8[n, L], "attention_mask": uint8[n, L]
         | None, "lengths": uint32[n]} with the tokenizer's pair truncation, pair template and padding applied on the device
         (what `encode_batch` on pairs + stacking the Encodings' ids / type_ids / attention_mask gives in the reference).
@@ -932,7 +969,8 @@ class Tokenizer:
         pair p, 2p + 1 the second.  A pair that cannot be truncated raises ValueError as the reference does.
         return_overflowing_tokens / return_offsets_mapping as in encode_batch_dense: a pair gives (1 + o_x)(1 + o_y) rows for
         the parts of its two sequences, in the reference's order; without return_overflowing_tokens a stride is refused
-        (UnsupportedConfig: it only shapes the overflowing parts)."""
+        (UnsupportedConfig: it only shapes the overflowing parts).  trim_offsets and the row metadata as in encode_batch_dense;
+        sequence ids are 0 for the pair's first sequence and 1 for its second, whatever the template order."""
         if doc_off is None:
             seqs = []
             for x in pairs:
@@ -944,7 +982,8 @@ class Tokenizer:
         doc_off = np.ascontiguousarray(doc_off, dtype=np.uint64)
         if len(doc_off) % 2 != 1:
             raise ValueError(f"a batch of n pairs has 2n + 1 document offsets, not {len(doc_off)}")
-        sp, keep = self.pair_dense_spec(add_special_tokens, want_mask, return_overflowing_tokens, return_offsets_mapping)
+        sp, keep = self.pair_dense_spec(add_special_tokens, want_mask, return_overflowing_tokens, return_offsets_mapping, trim_offsets,
+                                        return_special_tokens_mask, return_sequence_ids, return_word_ids)
         try:
             rows = self._dense_call("b2t_encode_pairs_dense", data, doc_off, (len(doc_off) - 1) // 2, sp, want_mask, True)
         except B2TError as ex:
