@@ -163,14 +163,14 @@ class BertNormalizer:
         if self.chinese:
             chars = [y for c, a, b in chars for y in (((0x20, a, b), (c, a, b), (0x20, a, b)) if self._chin[c] else ((c, a, b),))]
         if self.strip:
-            dec = []
+            dec = []                  # (code point, first piece of its character?)
             for c, a, b in chars:
                 if 0xAC00 <= c <= 0xD7A3:
                     si = c - 0xAC00
                     seq = [0x1100 + si // 588, 0x1161 + (si % 588) // 28] + ([0x11A7 + si % 28] if si % 28 else [])
                 else:
                     seq = self._nfd.get(c, [c])
-                dec += [(x, a, b) for x in seq]
+                dec += [(x, k == 0) for k, x in enumerate(seq)]
             # canonical ordering (UAX #15): runs of characters with a non-zero combining class are sorted by class, stably;
             # which characters have one is probed from the reference, the class values (stable across Unicode versions) are Python's
             ccc = lambda x: unicodedata.combining(chr(x)) if self._ccc[x] else 0
@@ -184,7 +184,17 @@ class BertNormalizer:
                     j += 1
                 dec[i:j] = sorted(dec[i:j], key=lambda t: ccc(t[0]))
                 i = j
-            chars = [(c, a, b) for c, a, b in dec if not self._mn[c]]
+            # NormalizedString::transform (normalizer.rs:347-412) hands the alignments out in the order it consumes the input, not
+            # with the code points: a first piece takes the next input character's, any other piece the last consumed one's
+            # ((0, 0) before the first).  A mark that sorting moved takes over another character's alignment.
+            out, k = [], 0
+            for x, first in dec:
+                if first:
+                    k += 1
+                al = chars[k - 1][1:] if k else (0, 0)
+                if not self._mn[x]:
+                    out.append((x,) + al)
+            chars = out
         if self.lower:
             chars = [(y, a, b) for c, a, b in chars for y in self._low.get(c, [c])]
         out, al = bytearray(), []

@@ -42,9 +42,28 @@ B2T_HDI uint32_t edge_hash(uint32_t node, uint32_t byte) {
 }
 
 // BertNormalizer table entries (norm_kernels.cuh NormTables.ent): kind in bits 0-1
-enum { NORM_IDENT = 0u, NORM_REMOVE = 1u, NORM_STRING = 2u, NORM_SURVIVOR = 3u, NORM_CCC_FLAG = 4u };
-// NORM_SURVIVOR: a character with a non-zero canonical combining class that strip_accents keeps (image = itself);
-// NORM_CCC_FLAG on a NORM_REMOVE entry: a dropped character with a combining class; on a NORM_SURVIVOR entry: never usable
+enum { NORM_IDENT = 0u, NORM_REMOVE = 1u, NORM_STRING = 2u, NORM_SURVIVOR = 3u, NORM_MARK_FLAG = 4u, NORM_TAIL_FLAG = 0x80u };
+constexpr uint32_t NORM_LEN_MASK = 31u;   // NORM_STRING: image bytes in bits 2-6 (at most 12), pool offset in bits 8-31
+// NORM_SURVIVOR: a character whose NFD starts with a non-zero canonical combining class and that strip_accents keeps
+// (image = itself).  Every other such character is NORM_REMOVE under strip_accents, so an IDENT or STRING character starts
+// with a class-0 character: no mark in front of it sorts past it.
+// NORM_MARK_FLAG on a NORM_REMOVE entry: canonical ordering sees through the removed character -- its NFD starts with a
+// non-zero class, or clean_text removes it before NFD runs and the characters on its two sides meet;
+// on a NORM_SURVIVOR entry: its image is not itself (no such character today), always refused.
+// NORM_TAIL_FLAG on a NORM_STRING entry: its decomposition keeps a character with a non-zero class behind its first
+// (U+1D15E -> U+1D157 U+1D165, 13 musical symbols): a mark right behind it can sort in front of that kept piece, which then
+// takes the mark's character.  The kernels check what follows it as they check a survivor's neighbours.
+
+// Can NFD's canonical ordering reach a kept mark across its neighbour cp (entry e; ascii: image of an ASCII character,
+// 0xFF = removed, which only clean_text does)?  Any other neighbour behind the mark starts with a class-0 character; any
+// other in front of it ends with a class-0 character or with pieces of its decomposition that strip_accents drops (a
+// NORM_TAIL_FLAG character checks its own look-ahead).  The mark may sort in front of dropped pieces, but they are not first
+// pieces and take no character's alignment in NormalizedString::transform, so it keeps its own and the text is the same.
+B2T_HDI bool norm_mark_neighbour(uint32_t cp, uint32_t e, const uint8_t* ascii) {
+  if (cp < 128u) return ascii[cp] == 0xFFu;
+  const uint32_t kind = e & 3u;
+  return kind == NORM_SURVIVOR || (kind == NORM_REMOVE && (e & NORM_MARK_FLAG) != 0u);
+}
 
 // Everything the model kernels need, passed by value.
 struct DeviceTables {

@@ -60,7 +60,7 @@ extern "C" int b2t_bert_normalizer_images(int32_t flags, uint8_t* pool, size_t c
     const uint32_t e = nh.ent[(size_t)nh.blk[c >> 7] * 128 + (c & 127)], kind = e & 3u;
     if (kind == NORM_REMOVE || (c >= 0xD800 && c <= 0xDFFF)) continue;
     uint8_t tmp[4]; const uint8_t* src = tmp; size_t len;
-    if (kind == NORM_STRING) { src = nh.pool.data() + (e >> 8); len = (e >> 2) & 63u; }
+    if (kind == NORM_STRING) { src = nh.pool.data() + (e >> 8); len = (e >> 2) & NORM_LEN_MASK; }
     else {   // the character itself
       if (c < 0x80) { tmp[0] = (uint8_t)c; len = 1; }
       else if (c < 0x800) { tmp[0] = 0xC0 | (c >> 6); tmp[1] = 0x80 | (c & 63); len = 2; }
@@ -715,8 +715,8 @@ static int normalize(b2t_engine* e, Workspace& ws, Batch& b, uint32_t flags, cud
   CU(cudaMemcpyAsync(h_tot, ws.nrm_tot.p, 24, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));   // one small read: the size of the normalized batch
   if ((uint32_t)h_tot[2] & ERR_NORM_UNSUPPORTED)
-    return fail(B2T_ERR_UNSUPPORTED, "the text holds a combining character that strip_accents keeps right behind another combining character: "
-                "their canonical order (NFD) is not restated on the device");
+    return fail(B2T_ERR_UNSUPPORTED, "the text holds a combining character that strip_accents keeps next to another combining character "
+                "or a removed one: their canonical order (NFD) is not restated on the device");
   const int64_t m = (int64_t)h_tot[0];
   if (m + (int64_t)n_docs >= (1ll << 31)) return fail(B2T_ERR_TOO_LARGE, "normalized batch of %lld bytes exceeds the per-call limit of 2^31-1; split it", (long long)m);
   if ((rc = ws.nrm_bytes.ensure((size_t)m + 64)) || (rc = ws.nrm_src_char.ensure(((size_t)m + 1) * 4))) return rc;

@@ -69,9 +69,11 @@ static void utf8_append(std::string& s, uint32_t cp);
 // BertNormalizer (normalizers/bert.rs:92-136) as a table: the image of every code point under the enabled steps, in the
 // reference's order clean_text -> handle_chinese_chars -> strip_accents (NFD, drop Mn) -> lowercase.  Every step maps one
 // character to a sequence of characters on its own; NFD's canonical reordering only moves characters with a non-zero
-// combining class (809 as the reference sees them, probed: tools/gen_bert_tables.py), and strip_accents drops 726 of them,
-// so composing per character is exact.  (83 newer characters with a combining class are NOT Mn for the reference and
-// survive: NORM_SURVIVOR, see norm_kernels.cuh.)
+// combining class (817 code points decompose to one first, as the reference sees them, probed: tools/gen_bert_tables.py),
+// and strip_accents drops 734 of them, so composing per character is exact for the text.  The alignment is not always:
+// NormalizedString hands the original characters out in input order, so a kept mark that sorting moves takes another
+// character's.  The 83 newer characters with a combining class that are NOT Mn for the reference survive: NORM_SURVIVOR,
+// refused where a neighbour lets canonical ordering reach them (norm_kernels.cuh norm_survivor_refused).
 void build_bert_norm(bool clean_text, bool chinese, bool strip_accents, bool lowercase, NormHost* out) {
   auto in_ranges = [](const uint32_t (*r)[2], uint32_t cnt, uint32_t c) {
     uint32_t lo = 0, hi = cnt;
@@ -93,8 +95,10 @@ void build_bert_norm(bool clean_text, bool chinese, bool strip_accents, bool low
       uint32_t e = NORM_IDENT;
       if (c < 0xD800 || c > 0xDFFF) {
         seq.assign(1, c);
+        bool cleaned = false;     // clean_text removes it: NFD never sees it
+        bool kept_mark = false;   // strip_accents keeps a piece of it with a non-zero class
         if (clean_text) {
-          if (in_ranges(B2T_BERT_REMOVE, B2T_BERT_REMOVE_COUNT, c)) seq.clear();
+          if (in_ranges(B2T_BERT_REMOVE, B2T_BERT_REMOVE_COUNT, c)) { seq.clear(); cleaned = true; }
           else if (in_ranges(B2T_BERT_TOSPACE, B2T_BERT_TOSPACE_COUNT, c)) seq.assign(1, 0x20u);
         }
         if (chinese && seq.size() == 1 && in_ranges(B2T_BERT_CHINESE, B2T_BERT_CHINESE_COUNT, seq[0])) { const uint32_t x = seq[0]; seq = {0x20u, x, 0x20u}; }
@@ -111,25 +115,31 @@ void build_bert_norm(bool clean_text, bool chinese, bool strip_accents, bool low
             }
           }
           seq.clear();
-          for (uint32_t x : tmp) if (!in_ranges(B2T_BERT_MN, B2T_BERT_MN_COUNT, x)) seq.push_back(x);
+          for (uint32_t x : tmp)
+            if (!in_ranges(B2T_BERT_MN, B2T_BERT_MN_COUNT, x)) {
+              seq.push_back(x);
+              kept_mark = kept_mark || in_ranges(B2T_BERT_CCC, B2T_BERT_CCC_COUNT, x);   // a kept piece with a non-zero class
+            }
         }
         if (lowercase) {
           tmp.clear();
           for (uint32_t x : seq) { auto it = low.find(x); if (it == low.end()) tmp.push_back(x); else tmp.insert(tmp.end(), it->second.begin(), it->second.end()); }
           seq.swap(tmp);
         }
-        const bool reorders = strip_accents && in_ranges(B2T_BERT_CCC, B2T_BERT_CCC_COUNT, c);   // non-zero combining class
-        if (seq.empty()) e = NORM_REMOVE | (reorders ? NORM_CCC_FLAG : 0u);
+        // NFD starts with a non-zero combining class: canonical ordering can move it (every such character NFD keeps is a
+        // NORM_SURVIVOR and every other one NORM_REMOVE, so IDENT and STRING characters start with class 0, b2t_tables.h)
+        const bool reorders = strip_accents && in_ranges(B2T_BERT_CCC, B2T_BERT_CCC_COUNT, c);
+        if (seq.empty()) e = NORM_REMOVE | (reorders || (strip_accents && cleaned) ? NORM_MARK_FLAG : 0u);
         else if (reorders) {
-          // one of the 83 characters with a combining class that strip_accents does not drop: its image is itself, but NFD
-          // may have to reorder it with a neighbouring mark -- the kernels refuse the batch if it FOLLOWS another such character
-          e = (seq.size() == 1 && seq[0] == c) ? NORM_SURVIVOR : (NORM_SURVIVOR | NORM_CCC_FLAG);
+          // one of the 83 characters with a combining class that strip_accents does not drop: its image is itself, but NFD may
+          // reorder it with a mark beside it -- the kernels refuse the batch when a neighbour lets it (norm_survivor_refused)
+          e = (seq.size() == 1 && seq[0] == c) ? NORM_SURVIVOR : (NORM_SURVIVOR | NORM_MARK_FLAG);
         } else if (!(seq.size() == 1 && seq[0] == c)) {
           img.clear();
           for (uint32_t x : seq) utf8_append(img, x);
           const size_t src_len = c < 0x80 ? 1 : (c < 0x800 ? 2 : (c < 0x10000 ? 3 : 4));
-          if (img.size() > 3 * src_len || img.size() > 62) out->ok = false;   // (norm_write_kernel sizes its staging for 3x; holds for every character today)
-          e = NORM_STRING | ((uint32_t)img.size() << 2) | ((uint32_t)out->pool.size() << 8);
+          if (img.size() > 3 * src_len || img.size() > NORM_LEN_MASK) out->ok = false;   // (norm_write_kernel sizes its staging for 3x; holds for every character today)
+          e = NORM_STRING | ((uint32_t)img.size() << 2) | ((uint32_t)out->pool.size() << 8) | (kept_mark ? NORM_TAIL_FLAG : 0u);
           out->pool.insert(out->pool.end(), img.begin(), img.end());
         }
         if (c < 128) out->ascii[c] = seq.empty() ? 0xFF : (uint8_t)seq[0];   // (an ASCII character's image is one ASCII character; 0xFF = dropped)

@@ -8,10 +8,12 @@
 // Every step of BertNormalizer maps ONE character to a (possibly empty) sequence of characters without looking at its
 // neighbours, so the whole normalizer is a table: code point -> UTF-8 bytes of its image (host_tables.cu composes it
 // from the probed per-character facts of bert_tables.inc for the four flags).  The one context-dependent part of NFD,
-// canonical reordering of combining marks, only permutes characters that strip_accents then drops: all 809 characters with
-// a non-zero combining class but 83 count as Mn for the reference (probed, tools/gen_bert_tables.py).  One of those 83 right
-// behind another combining character is the only place where order could matter: such a batch is refused (ERR_NORM_UNSUPPORTED
-// -> B2T_ERR_UNSUPPORTED), never normalized differently.
+// canonical reordering of combining marks, mostly permutes characters that strip_accents then drops: of the 817 characters
+// whose NFD starts with a non-zero combining class all but 83 are removed (probed, tools/gen_bert_tables.py).  Order still
+// matters for the alignment of the 83 survivors: NormalizedString hands the original characters out in input order, so a
+// survivor that sorting moves past a mark -- in front of it or behind it, also one that clean_text removed between them --
+// takes that mark's character.  A survivor with a neighbour that lets canonical ordering reach it is refused
+// (norm_survivor_refused: ERR_NORM_UNSUPPORTED -> B2T_ERR_UNSUPPORTED), never aligned differently.
 //
 //   N1 norm_count   per 2 KB page of the ORIGINAL batch: bytes of its image, characters it holds
 //   (exclusive scans of both, one host read of the total)
@@ -36,24 +38,47 @@ constexpr int NORM_PER_THREAD = PAGE / NORM_THREADS;   // 8 bytes
 
 struct NormTables {
   const uint16_t* blk;      // [0x110000 >> 7]: block of the code point
-  const uint32_t* ent;      // [blocks][128]: kind (bits 0-1) | byte length (bits 2-7) | pool offset (bits 8-31)
+  const uint32_t* ent;      // [blocks][128]: kind (bits 0-1) | flags | byte length (bits 2-6) | pool offset (bits 8-31), b2t_tables.h
   const uint8_t* pool;      // UTF-8 images
   const uint8_t* ascii;     // [128]: image of an ASCII character (always one ASCII character), 0xFF = dropped
 };
 
-__device__ __forceinline__ uint32_t norm_entry(const NormTables& T, uint32_t cp) {
-  return __ldg(T.ent + (uint32_t)__ldg(T.blk + (cp >> 7)) * 128u + (cp & 127u));
+__host__ __device__ inline uint32_t norm_entry(const NormTables& T, uint32_t cp) {
+  return T.ent[(uint32_t)T.blk[cp >> 7] * 128u + (cp & 127u)];
 }
 
 // the character that starts at p (a lead byte): code point and byte length (bytes past the end read as 0)
-__device__ __forceinline__ uint32_t norm_decode(const uint8_t* __restrict__ b, int64_t p, int64_t n, int* len) {
-  const uint32_t b0 = __ldg(b + p);
+__host__ __device__ inline uint32_t norm_decode(const uint8_t* b, int64_t p, int64_t n, int* len) {
+  const uint32_t b0 = b[p];
   if (b0 < 0x80u) { *len = 1; return b0; }
   const int l = b0 < 0xE0u ? 2 : (b0 < 0xF0u ? 3 : 4);
   uint32_t cp = b0 & (0x7Fu >> l);
-  for (int k = 1; k < l; ++k) cp = (cp << 6) | (p + k < n ? (__ldg(b + p + k) & 0x3Fu) : 0u);
+  for (int k = 1; k < l; ++k) cp = (cp << 6) | (p + k < n ? (b[p + k] & 0x3Fu) : 0u);
   *len = l;
   return cp < 0x110000u ? cp : 0x10FFFFu;
+}
+
+// The character at byte p of the batch bytes[0, n) is a survivor or keeps a mark behind its first piece (NORM_TAIL_FLAG):
+// refused unless its image is itself (a survivor) and neither the character in front of it (a survivor) nor the one behind it
+// lets canonical ordering reach its kept mark (norm_mark_neighbour).  Then NFD leaves the mark where it is -- behind the
+// class-0 character before it, in front of anything it could change places with -- and NormalizedString aligns it with its
+// own character, as the image table does.  The neighbours are read in the packed batch, so a mark at a document edge looks
+// across it (a needless refusal at worst); the batch's ends stop the look.
+__host__ __device__ inline bool norm_survivor_refused(const uint8_t* bytes, int64_t p, int64_t n, const NormTables& T, const uint8_t* ascii) {
+  int len, l2;
+  const uint32_t e = norm_entry(T, norm_decode(bytes, p, n, &len));
+  if ((e & 3u) == NORM_SURVIVOR && (e & NORM_MARK_FLAG)) return true;
+  if ((e & 3u) == NORM_SURVIVOR && p > 0) {
+    int64_t q = p - 1;
+    while (q > 0 && (bytes[q] & 0xC0u) == 0x80u && p - q < 4) --q;
+    const uint32_t cp = norm_decode(bytes, q, n, &l2);
+    if (norm_mark_neighbour(cp, norm_entry(T, cp), ascii)) return true;
+  }
+  if (p + len < n) {
+    const uint32_t cp = norm_decode(bytes, p + len, n, &l2);
+    if (norm_mark_neighbour(cp, norm_entry(T, cp), ascii)) return true;
+  }
+  return false;
 }
 
 // block-wide exclusive scan of one int per thread (256 threads); returns the exclusive prefix, *total = block sum
@@ -117,7 +142,7 @@ __device__ __forceinline__ void norm_load_chunk(const uint8_t* __restrict__ byte
   }
   const int valid = n - base >= NORM_PER_THREAD ? NORM_PER_THREAD : (int)(n - base);
   uint32_t cps[NORM_PER_THREAD], clen[NORM_PER_THREAD], blk[NORM_PER_THREAD];
-  uint32_t lead = 0u, hi = 0u;   // bit i: byte i starts a character / a non-ASCII character
+  uint32_t lead = 0u, hi = 0u, surv = 0u;   // bit i: byte i starts a character / a non-ASCII character / one with a kept mark
 #pragma unroll
   for (int i = 0; i < NORM_PER_THREAD; ++i) {
     const uint32_t b0 = ((i < 4 ? c.w0 : c.w1) >> (8 * (i & 3))) & 0xFFu;
@@ -141,26 +166,16 @@ __device__ __forceinline__ void norm_load_chunk(const uint8_t* __restrict__ byte
       if (!((hi >> i) & 1u)) len = s_ascii[cps[i]] != 0xFFu ? 1u : 0u;
       else {
         const uint32_t e = c.ent[i], kind = e & 3u;
-        len = kind == NORM_REMOVE ? 0u : (kind == NORM_STRING ? ((e >> 2) & 63u) : clen[i]);
-        if (kind == NORM_SURVIVOR) {
-          // a combining character that survives strip_accents: NFD would have to order it against the combining character in
-          // front of it, if there is one (dropped or not) -- that case is refused, everything else is the identity
-          bool bad = (e & NORM_CCC_FLAG) != 0u;
-          const int64_t p = base + i;
-          if (p > 0) {
-            int64_t q = p - 1;
-            while (q > 0 && (__ldg(bytes + q) & 0xC0u) == 0x80u && p - q < 4) --q;
-            int l2;
-            const uint32_t e2 = norm_entry(T, norm_decode(bytes, q, n, &l2));
-            bad = bad || (e2 & 3u) == NORM_SURVIVOR || ((e2 & 3u) == NORM_REMOVE && (e2 & NORM_CCC_FLAG));
-          }
-          if (bad) atomicOr(err, ERR_NORM_UNSUPPORTED);
-        }
+        len = kind == NORM_REMOVE ? 0u : (kind == NORM_STRING ? ((e >> 2) & NORM_LEN_MASK) : clen[i]);
+        if (kind == NORM_SURVIVOR || (kind == NORM_STRING && (e & NORM_TAIL_FLAG))) surv |= 1u << i;
       }
       c.n_out += (int)len;
     }
     c.lens |= (unsigned long long)len << (6 * i);
   }
+  // kept marks are rare: one copy of the check serves them all, outside the unrolled loop
+  for (; surv; surv &= surv - 1u)
+    if (norm_survivor_refused(bytes, base + __ffs(surv) - 1, n, T, s_ascii)) atomicOr(err, ERR_NORM_UNSUPPORTED);
 }
 
 // ------------------------------------------------------------------------------------------------ N1
