@@ -946,7 +946,10 @@ __global__ void __launch_bounds__(TSCAN) tile_scan_top_kernel(unsigned long long
   if (threadIdx.x == 0) *total = s_run;
 }
 
-// one warp per page: provisional slots -> final CSR positions
+// one warp per page: provisional slots -> final CSR positions.  A page has a few hundred tokens, so a warp copies only
+// a dozen rounds of 32; each lane issues COMPACT_UNROLL rounds of loads before their stores, else every round waits for
+// its loads and the copy is bound by memory latency rather than bandwidth.
+constexpr int COMPACT_UNROLL = 8;
 __global__ void compact_kernel(const uint32_t* __restrict__ tile_count, const uint32_t* __restrict__ tile_first,
                                const unsigned long long* __restrict__ local_excl, const unsigned long long* __restrict__ block_excl, int64_t n_tiles,
                                const uint32_t* __restrict__ t_ids, const uint2* __restrict__ t_off, const uint32_t* __restrict__ t_wid,
@@ -955,12 +958,28 @@ __global__ void compact_kernel(const uint32_t* __restrict__ tile_count, const ui
   const int lane = threadIdx.x & 31;
   if (t >= n_tiles) return;
   const uint32_t cnt = tile_count[t];
-  if (!cnt) return;
   const unsigned long long src = tile_first[t], dst = local_excl[t] + block_excl[t / TSCAN];
-  for (uint32_t j = lane; j < cnt; j += 32) {
-    ids[dst + j] = t_ids[src + j];
-    if (off) off[dst + j] = t_off[src + j];
-    if (wid) wid[dst + j] = t_wid[src + j];
+  for (uint32_t j0 = lane; j0 < cnt; j0 += 32 * COMPACT_UNROLL) {
+    uint32_t a[COMPACT_UNROLL], w[COMPACT_UNROLL];
+    uint2 o[COMPACT_UNROLL];
+#pragma unroll
+    for (int u = 0; u < COMPACT_UNROLL; ++u) {
+      const uint32_t j = j0 + 32 * u;
+      if (j < cnt) {
+        a[u] = t_ids[src + j];
+        if (off) o[u] = t_off[src + j];
+        if (wid) w[u] = t_wid[src + j];
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < COMPACT_UNROLL; ++u) {
+      const uint32_t j = j0 + 32 * u;
+      if (j < cnt) {
+        ids[dst + j] = a[u];
+        if (off) off[dst + j] = o[u];
+        if (wid) wid[dst + j] = w[u];
+      }
+    }
   }
 }
 
