@@ -261,8 +261,9 @@ const uint8_t* b2t_result_type_ids(const b2t_result* r);
 
 /* Replaces PreTokenizer::pre_tokenize (tokenizer/mod.rs:65-67) for a batch: the splits of every document as
  * (start, end) BYTE offsets into the document (offsets[2k], offsets[2k+1]); row_ptr delimits documents.  ids and
- * word_ids are absent.  Host buffers in, pinned host buffers out.  (With add_prefix_space the split that contains the
- * inserted space starts at the first byte of the document.) */
+ * word_ids are absent.  Host buffers in, pinned host buffers out.  The text as given is split: the engine's normalizer
+ * and added tokens do not apply.  (With add_prefix_space the split that contains the inserted space starts at the
+ * first byte of the document.) */
 int b2t_pre_tokenize_batch(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs,
                            b2t_result** out);
 

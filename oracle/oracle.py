@@ -326,10 +326,14 @@ class Oracle:
 
     def pre_tokenize(self, doc):
         """[(start_byte, end_byte)] in original bytes, like pre_tokenize_str's offsets but in bytes."""
-        b = np.frombuffer(doc.encode("utf-8"), dtype=np.uint8)
+        return [tuple(s) for s in self.pre_tokenize_bytes(doc.encode("utf-8")).tolist()]
+
+    def pre_tokenize_bytes(self, raw):
+        """pre_tokenize of one document given as UTF-8 bytes -> np.uint32[k, 2] (for long documents)"""
+        b = np.frombuffer(raw, dtype=np.uint8)
         out = np.zeros(2 * (len(b) + 2), dtype=np.uint32)
         k = lib().orc_pretokenize(self._h, b.ctypes.data if b.size else 0, len(b), out.ctypes.data, len(b) + 2)
-        return [(int(out[2 * i]), int(out[2 * i + 1])) for i in range(k)]
+        return out[:2 * k].reshape(-1, 2)
 
 
 def dense_rows(ids, row_ptr, *, length, pad_to_multiple_of, max_length, pad_id, truncate_left, pad_left, pre, post):

@@ -385,6 +385,52 @@ def page_slots(probes, deltas=DELTAS):
     return slots
 
 
+def scan_block_slots(probes):
+    """around the 2 MiB boundaries of the page and tile scans (1024 pages): one probe per boundary"""
+    import random
+    rng = random.Random(3)
+    out = []
+    for m, probe in enumerate(probes, start=1):
+        out.append((probe, m * (2 << 20) + rng.choice([-2, -1, 0, 1, 2]), rng.choice(["start", "end"])))
+    return out
+
+
+# probes of the page-edge tests: pre-tokens whose length or content changes the scan's or the model's code path
+WIDE = {1: "abcdefghij", 2: "éßжяλ", 3: "中文語あア", 4: "𝒜𝒷𝓬𐐀𐐨"}   # letters (\p{L}) of 1..4 bytes
+
+
+def word(rng, n_bytes, width):
+    """a run of letters of exactly n_bytes, made of `width`-byte characters (ASCII letters first for the remainder)"""
+    r = n_bytes % width
+    return "".join(rng.choice(WIDE[1]) for _ in range(r)) + "".join(rng.choice(WIDE[width]) for _ in range(n_bytes // width))
+
+
+def bpe_probes():
+    import random
+    rng = random.Random(1)
+    out = [word(rng, n, w) for n in (16, 17, 24, 25, 32, 33, 255, 256, 257) for w in (1, 2, 3, 4)]
+    out += [" " * 40 + "x", "\n" * 33 + "x", " \t" * 20, "x" + " " * 33, "x   \n  y"]          # whitespace runs (\s+(?!\S))
+    out += ["don's", "it'S", "we'll", "x''s"]                                              # a contraction split by the edge
+    out += ["1" * n for n in (2, 3, 4, 5, 6, 7, 8, 9, 10)]                                 # Llama-3 digit runs of 3k-1, 3k, 3k+1
+    out += ["!?!...\r\n\r\nx", "--\r\n", ")]}\r\n\r\n\r\n"]                               # punctuation run + \r\n
+    out += ["", "x", "é"]                                                                    # empty and 1-character documents
+    return out
+
+
+def wordpiece_probes(max_chars):
+    import random
+    rng = random.Random(2)
+    out = []
+    for n in (max_chars - 1, max_chars, max_chars + 1):
+        out += ["".join(rng.choice("abcdefghijklmnop") for _ in range(n)), "".join(rng.choice(WIDE[4]) for _ in range(n))]
+    out += ["a" * max_chars, "𝒜" * max_chars, " " * 40 + "x", "x" + "\t" * 33, "don's", "", "x", "é"]
+    return out
+
+
+# characters the BertNormalizer expands: Hangul (three jamo with strip_accents), CJK (spaces around it), accents
+BERT_PROBES = ["".join(chr(0xAC00 + (37 * i) % 11172) for i in range(k)) for k in (5, 40, 90)] + ["中文字" * 12, "x中y", "ÀÉÎÕÜ" * 8, "ǅİ"]
+
+
 _exp = {}
 
 

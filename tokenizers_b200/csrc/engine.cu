@@ -686,10 +686,11 @@ static int repack_prefix(b2t_engine* e, Workspace& ws, Batch& b, cudaStream_t st
 }
 
 // N1-N2 BertNormalizer as a byte-rewriting pre-pass: the kernels after it see the normalized batch, the offsets are mapped
-// back at the end (N3 in finish_device); costs one small host sync for the size of the normalized batch
+// back at the end (N3 in finish_device); costs one small host sync for the size of the normalized batch.  Not for the
+// PreTokenizer seam (RUN_PRETOK): a PreTokenizer splits the text it is given, and the seam's offsets index that text.
 static int normalize(b2t_engine* e, Workspace& ws, Batch& b, uint32_t flags, cudaStream_t st) {
   ws.norm_active = false;
-  if (!e->norm_on || b.n == 0 || b.n_docs == 0) return B2T_OK;
+  if (!e->norm_on || ws.req.until == RUN_PRETOK || b.n == 0 || b.n_docs == 0) return B2T_OK;
   const uint8_t* d_bytes = b.bytes; const uint64_t* d_doc_off = b.doc_off; const int64_t n = b.n; const uint32_t n_docs = b.n_docs;
   int rc;
   if (flags & B2T_OFFSETS_BYTES) return fail(B2T_ERR_UNSUPPORTED, "byte offsets are not available behind a normalizer (character offsets are)");
@@ -1520,8 +1521,9 @@ extern "C" int b2t_encode_pairs_dense(b2t_engine* e, const uint8_t* bytes, const
                    [&](b2t_engine::SlotSet& ss, uint32_t dq_flags) { return host_encode(e, ss, bytes, doc_off, n_docs, 0u, out, &dq, dq_flags); });
 }
 
-// PreTokenizer seam: runs K0/K1 and expands the split bitmaps into (start, end) pairs.  The expansion of the bitmap
-// into the pair list is output formatting and happens on the host (this is an inspection API, not the hot path).
+// PreTokenizer seam: runs K0/K1 on the text as given (neither the normalizer nor the added tokens apply) and expands the
+// split bitmaps into (start, end) pairs.  The expansion of the bitmap into the pair list is output formatting and
+// happens on the host (this is an inspection API, not the hot path).
 static int pre_tokenize(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, b2t_result** out) {
   const uint64_t n = doc_off[n_docs];
   Workspace& ws = ss.slot[0];
@@ -1539,19 +1541,24 @@ static int pre_tokenize(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* b
   CU(cudaStreamSynchronize(ws.stream));
   b2t_result* r = pool_get(e);
   r->eng = e; r->on_device = 0; r->n_docs = n_docs;
+  if ((rc = r->h_row_ptr.ensure(((size_t)n_docs + 1) * 8, false))) { pool_put(e, r); return rc; }
   auto bit = [](const std::vector<uint32_t>& v, uint64_t p) { return (v[p >> 5] >> (p & 31)) & 1u; };
-  uint64_t count = 0;
-  for (uint64_t p = 0; p < n_eff; ++p) count += bit(sb, p) && !bit(db, p);
-  if ((rc = r->h_offsets.ensure((count + 1) * 8, false)) || (rc = r->h_row_ptr.ensure(((size_t)n_docs + 1) * 8, false))) { pool_put(e, r); return rc; }
-  uint32_t* off = r->h_offsets.as<uint32_t>();
+  // one walk over each document's range of the batch the kernels ran on both counts the splits and writes them, so the
+  // bitmaps are never read outside that batch and the pairs never outgrow their buffer
+  std::vector<uint32_t> pairs;
   uint64_t* rp = r->h_row_ptr.as<uint64_t>();
-  uint64_t k = 0, shift = 0;
+  uint64_t shift = 0;
   for (uint32_t d = 0; d < n_docs; ++d) {
-    rp[d] = k;
+    rp[d] = pairs.size() / 2;
     const uint64_t len = doc_off[d + 1] - doc_off[d];
     const bool pre = e->add_prefix_space && len > 0 && bytes[doc_off[d]] != ' ';
     const uint64_t dstart = doc_off[d] + shift;          // start of the document in the (re-packed) device batch
     const uint64_t end = dstart + len + (pre ? 1 : 0);
+    if (end > n_eff) {
+      pool_put(e, r);
+      return fail(B2T_ERR_CUDA, "internal error: document %u ends at byte %llu of a pre-tokenized batch of %llu bytes", d,
+                  (unsigned long long)end, (unsigned long long)n_eff);
+    }
     uint64_t first_len = 1;                               // bytes of the first original character
     if (pre) { while (first_len < len && (bytes[doc_off[d] + first_len] & 0xC0) == 0x80) ++first_len; }
     uint64_t p = dstart;
@@ -1561,13 +1568,17 @@ static int pre_tokenize(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* b
       if (!bit(db, p)) {
         uint64_t a = p - dstart, b = q - dstart;
         if (pre) { b = (b == 1) ? first_len : b - 1; a = a ? a - 1 : 0; }  // the inserted space is aligned to the first character
-        off[2 * k] = (uint32_t)a; off[2 * k + 1] = (uint32_t)b; ++k;
+        pairs.push_back((uint32_t)a); pairs.push_back((uint32_t)b);
       }
       p = q;
     }
     if (pre) ++shift;
   }
+  const uint64_t k = pairs.size() / 2;
   rp[n_docs] = k;
+  if ((rc = r->h_offsets.ensure((k + 1) * 8, false))) { pool_put(e, r); return rc; }
+  uint32_t* off = r->h_offsets.as<uint32_t>();
+  if (k) memcpy(off, pairs.data(), k * 8);
   r->n_tokens = k; r->ids = nullptr; r->word_ids = nullptr; r->offsets = off; r->row_ptr = rp;
   *out = r;
   return B2T_OK;

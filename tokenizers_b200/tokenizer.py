@@ -1183,7 +1183,8 @@ class Tokenizer:
         return [self.decode(s, skip_special_tokens) for s in sequences]
 
     def pre_tokenize_batch(self, docs):
-        """PreTokenizer seam: per document the list of (start_byte, end_byte) of its splits."""
+        """PreTokenizer seam: per document the list of (start_byte, end_byte) of its splits of the text as given (the
+        normalizer and the added tokens do not apply, as with the reference's `pre_tokenizer.pre_tokenize_str`)."""
         data, off = _pack(docs, np.uint64)
         n = len(off) - 1
         L = _lib.lib()
