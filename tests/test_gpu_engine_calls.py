@@ -1,6 +1,7 @@
 """GPU (-m gpu): the host-side call paths of the engine (csrc/engine.cu) that the encode tests do not reach on their own:
 the rerun with a grown long pool at every entry point, the begin / finish split of the device-resident entry point on
-one GPU, the per-kernel profiling record, and the argument checks of the host-buffer and device-resident entry points."""
+one GPU, the views of a result the pool hands out again, the per-kernel profiling record, and the argument checks of the
+host-buffer and device-resident entry points."""
 import ctypes
 import numpy as np
 import pytest
@@ -166,6 +167,38 @@ def test_finish_refusals():
                                                ctypes.byref(n_tok)))
     assert L.b2t_encode_batch_device_finish(tok.handle, p, None, p, p, 0, None) == _lib.B2T_ERR_INVALID
     assert b"d_offsets is null" in L.b2t_last_error()
+
+
+# ---------------------------------------------------------------------------------------------- pooled results
+DENSE_VIEWS = ["b2t_result_dense_ids", "b2t_result_attention_mask", "b2t_result_row_lengths", "b2t_result_type_ids", "b2t_result_row_sample",
+               "b2t_result_dense_offsets", "b2t_result_special_tokens_mask", "b2t_result_sequence_ids", "b2t_result_dense_word_ids"]
+
+
+def test_pooled_result_has_no_stale_dense_views():
+    """A host dense result freed back to the engine's pool is the one the next host call gets (the pool is LIFO): a
+    b2t_pre_tokenize_batch result then has no dense rows, as include/b2t.h promises for results that are not dense"""
+    from tokenizers_b200 import Tokenizer
+    _lib, L = lib()
+    tok = Tokenizer.from_str(helpers.asset_json("gpt2_style"))
+    tok.enable_truncation(16)
+    tok.enable_padding(length=16)
+    sp, keep = tok.dense_spec(add_special_tokens=False, want_mask=True)
+    data, off = corpus.generate(2, 46, 0, 20)
+    n = len(off) - 1
+    res = ctypes.c_void_p()
+    _lib.check(L.b2t_encode_batch_dense(tok.handle, data.ctypes.data, off.ctypes.data, n, ctypes.byref(sp), ctypes.byref(res)))
+    assert L.b2t_result_dense_length(res) == 16 and L.b2t_result_attention_mask(res)
+    dense = res.value
+    L.b2t_result_free(res)
+    res = ctypes.c_void_p()
+    _lib.check(L.b2t_pre_tokenize_batch(tok.handle, data.ctypes.data, off.ctypes.data, n, ctypes.byref(res)))
+    try:
+        assert res.value == dense
+        assert L.b2t_result_dense_length(res) == 0 and L.b2t_result_dense_rows(res) == 0
+        assert [f for f in DENSE_VIEWS if getattr(L, f)(res) is not None] == []
+    finally:
+        L.b2t_result_free(res)
+    del keep
 
 
 # ---------------------------------------------------------------------------------------------- profiling record

@@ -138,6 +138,28 @@ struct DenseReq {
   uint32_t L() const { return pairs() ? P.L : S.L; }
 };
 
+// The outputs of dense mode: the bytes of one element, one element per cell of the [R, L] rows or per row, and what in
+// the request asks for it.  The workspace, the pinned result and the result's views hold one buffer per output.
+enum DenseOut { OUT_IDS, OUT_MASK, OUT_LEN, OUT_TYPE, OUT_SAMPLE, OUT_OFF, OUT_SPECIAL, OUT_SEQ, OUT_WORD, N_DENSE_OUT };
+struct DenseOutput {
+  uint32_t elem;
+  bool per_row;
+  bool (*wanted)(const DenseReq&);
+};
+constexpr DenseOutput DENSE_OUT[N_DENSE_OUT] = {
+    {4, false, [](const DenseReq&) { return true; }},               // ids
+    {1, false, [](const DenseReq& q) { return q.want_mask; }},      // attention mask
+    {4, true, [](const DenseReq&) { return true; }},                // row lengths
+    {1, false, [](const DenseReq& q) { return q.pairs(); }},        // type ids
+    {4, true, [](const DenseReq& q) { return q.overflow; }},        // row sample: the input of each row
+    {8, false, [](const DenseReq& q) { return q.offsets; }},        // offset rows: (start, end)
+    {1, false, [](const DenseReq& q) { return q.special_mask; }},   // special-tokens mask
+    {1, false, [](const DenseReq& q) { return q.seq_ids; }},        // sequence ids
+    {4, false, [](const DenseReq& q) { return q.word_ids; }},       // word ids
+};
+// the bytes of one row of output k
+static size_t dense_row_bytes(int k, uint32_t L) { return DENSE_OUT[k].per_row ? DENSE_OUT[k].elem : (size_t)DENSE_OUT[k].elem * L; }
+
 // How far run_device_pipeline goes: pre-tokenization only (K0..K1b), up to the token count (the caller finishes into its
 // own buffers), or the whole result in the workspace.
 enum RunUntil { RUN_PRETOK, RUN_COUNT, RUN_RESULT };
@@ -167,9 +189,8 @@ struct Workspace {
   DevBuf page_long, long_desc, long_desc1, soft_bits, page_soft, lp_id, lp_val, lp_len, lp_plen, lp_aux, lp_out;  // long BPE pre-tokens (long_kernels.cuh)
   unsigned long long pool_cap = 0;
   DevBuf wcache;                      // per-batch word cache (model_kernels.cuh)
-  DevBuf dense_ids, dense_mask, dense_len, dense_type;  // dense [n_rows, L] rows (dense_kernels.cuh); type ids: pairs only
-  DevBuf dense_off, row_count, row_lexcl, row_bsum, row_base, row_sample;  // overflow rows: offset rows, the count pass and its scan
-  DevBuf dense_special, dense_seq, dense_word;   // row metadata: special-tokens mask, sequence ids, word ids
+  DevBuf dense[N_DENSE_OUT];           // dense rows (dense_kernels.cuh), one buffer per DenseOut
+  DevBuf row_count, row_lexcl, row_bsum, row_base;   // overflow rows: the count pass, its scan and each input's first row
   // BertNormalizer pre-pass (norm_kernels.cuh): the normalized batch and what maps its tokens back to the original
   DevBuf nrm_doc_bits, nrm_pfd, nrm_page_out, nrm_page_chars, nrm_lexcl_o, nrm_bsum_o, nrm_lexcl_c, nrm_bsum_c, nrm_tot, nrm_bytes, nrm_src_char, nrm_doc_off, nrm_doc_char0;
   bool norm_active = false;
@@ -190,18 +211,24 @@ struct b2t_result {
   int on_device = 0;
   uint32_t n_docs = 0;
   uint64_t n_tokens = 0;
-  const uint32_t* ids = nullptr; const uint32_t* offsets = nullptr; const uint32_t* word_ids = nullptr; const uint64_t* row_ptr = nullptr;
+  struct Views {   // what the accessors return: all null / 0 in a result the pool hands out
+    const uint32_t* ids = nullptr; const uint32_t* offsets = nullptr; const uint32_t* word_ids = nullptr; const uint64_t* row_ptr = nullptr;
+    // dense mode (b2t_encode_batch_dense*, b2t_encode_pairs_dense*): [n_rows, dense_len] rows instead of the CSR (n_docs =
+    // pairs for a pair result; n_rows = n_docs without overflowing parts)
+    uint32_t dense_len = 0, n_rows = 0;
+    const void* dense[N_DENSE_OUT] = {};
+  } view;
   PinBuf h_ids, h_offsets, h_word_ids, h_row_ptr;  // host results own pinned memory (returned to the engine pool on free)
-  // dense mode (b2t_encode_batch_dense*, b2t_encode_pairs_dense*): [n_docs, dense_len] rows instead of the CSR (n_docs =
-  // pairs for a pair result, which also has type ids)
-  uint32_t dense_len = 0;
-  const uint32_t* dense_ids = nullptr; const uint8_t* dense_mask = nullptr; const uint32_t* row_len = nullptr;
-  const uint8_t* type_ids = nullptr;
-  uint32_t n_rows = 0;   // dense rows R (n_docs without overflowing parts)
-  const uint32_t* row_sample = nullptr; const uint32_t* dense_off = nullptr;
-  const uint8_t* special_mask = nullptr; const int8_t* seq_ids = nullptr; const uint32_t* dense_word = nullptr;
-  PinBuf h_dense_ids, h_dense_mask, h_row_len, h_type_ids, h_row_sample, h_dense_off, h_special, h_seq, h_word;
+  PinBuf h_dense[N_DENSE_OUT];
 };
+
+// Publishes the dense views of a finished result: output k at buf[k] (the workspace's or the pinned result's buffers)
+// where the request asks for it.
+template <class Buf>
+static void set_dense_views(b2t_result* r, const DenseReq& dq, uint32_t n_rows, const Buf (&buf)[N_DENSE_OUT]) {
+  r->view.dense_len = dq.L(); r->view.n_rows = n_rows;
+  for (int k = 0; k < N_DENSE_OUT; ++k) r->view.dense[k] = DENSE_OUT[k].wanted(dq) ? buf[k].p : nullptr;
+}
 
 constexpr int NSLOT = 3;   // chunk workspaces of one host-path call: NSLOT - 1 chunks are in flight while the next is issued
 constexpr int MAX_KERNEL_RECORDS = 16;
@@ -463,6 +490,20 @@ static int dense_engine_flags(const b2t_engine* e, const DenseReq& dq, uint32_t*
   return B2T_OK;
 }
 
+// The tail both spec readers share, after the template: the length budget left beside its n_special tokens (*budget) and
+// how rows are padded.  dq->docs_per_row is set.
+template <class Spec>
+static int dense_length(const Spec* sp, uint32_t n_special, uint32_t* budget, DenseReq* dq) {
+  // tokenizer/mod.rs:1272-1283: the sequence (or the pair) is truncated to max_length - n_added_tokens
+  if (sp->max_length && sp->max_length < n_special) return fail(B2T_ERR_INVALID, "max_length %u is smaller than the %u special tokens of the template", sp->max_length, n_special);
+  *budget = sp->max_length ? sp->max_length - n_special : DENSE_NO_LIMIT;
+  dq->batch_longest = sp->length == 0;
+  dq->multiple = sp->pad_to_multiple_of;
+  dq->L() = dq->batch_longest ? 0u : dense_round(sp->length, dq->multiple);
+  dq->want_mask = sp->want_mask != 0;
+  return B2T_OK;
+}
+
 // b2t_dense_spec -> DenseReq, checked
 static int make_dense_req(const b2t_dense_spec* sp_in, DenseReq* dq) {
   if (!sp_in) return fail(B2T_ERR_INVALID, "dense spec is null");
@@ -474,20 +515,12 @@ static int make_dense_req(const b2t_dense_spec* sp_in, DenseReq* dq) {
   if (sp->n_pre > (uint32_t)DENSE_MAX_SPECIAL || sp->n_post > (uint32_t)DENSE_MAX_SPECIAL)
     return fail(B2T_ERR_UNSUPPORTED, "templates with more than %d special tokens on one side are not supported", DENSE_MAX_SPECIAL);
   if ((sp->n_pre && !sp->pre_ids) || (sp->n_post && !sp->post_ids)) return fail(B2T_ERR_INVALID, "dense spec: null special-token list");
-  const uint32_t n_special = sp->n_pre + sp->n_post;
-  // tokenizer/mod.rs:1272-1283: the sequence is truncated to max_length - n_added_tokens
-  if (sp->max_length && sp->max_length < n_special) return fail(B2T_ERR_INVALID, "max_length %u is smaller than the %u special tokens of the template", sp->max_length, n_special);
   memset(&dq->S, 0, sizeof(dq->S));
-  dq->S.keep_max = sp->max_length ? sp->max_length - n_special : DENSE_NO_LIMIT;
   dq->S.pad_id = sp->pad_id; dq->S.n_pre = sp->n_pre; dq->S.n_post = sp->n_post;
   dq->S.trunc_left = sp->truncate_left ? 1 : 0; dq->S.pad_left = sp->pad_left ? 1 : 0;
   for (uint32_t i = 0; i < sp->n_pre; ++i) dq->S.pre[i] = sp->pre_ids[i];
   for (uint32_t i = 0; i < sp->n_post; ++i) dq->S.post[i] = sp->post_ids[i];
-  dq->batch_longest = sp->length == 0;
-  dq->multiple = sp->pad_to_multiple_of;
-  dq->S.L = dq->batch_longest ? 0u : dense_round(sp->length, dq->multiple);
-  dq->want_mask = sp->want_mask != 0;
-  return B2T_OK;
+  return dense_length(sp, sp->n_pre + sp->n_post, &dq->S.keep_max, dq);
 }
 // b2t_pair_dense_spec -> DenseReq (pairs), checked: the piece list is split into pre X mid Y post
 static int make_dense_req(const b2t_pair_dense_spec* sp_in, DenseReq* dq) {
@@ -528,107 +561,64 @@ static int make_dense_req(const b2t_pair_dense_spec* sp_in, DenseReq* dq) {
   for (uint32_t i = 0; i < n_seg[1]; ++i) P.special[n_seg[0] + i] = P.special[DENSE_MAX_SPECIAL + i];
   for (uint32_t i = 0; i < n_seg[2]; ++i) P.special[n_seg[0] + n_seg[1] + i] = P.special[2 * DENSE_MAX_SPECIAL + i];
   P.n_pre = n_seg[0]; P.n_mid = n_seg[1]; P.n_post = n_seg[2];
-  const uint32_t n_special = P.n_pre + P.n_mid + P.n_post;
-  // tokenizer/mod.rs:1272-1283: the pair is truncated to max_length - n_added_tokens
-  if (sp->max_length && sp->max_length < n_special) return fail(B2T_ERR_INVALID, "max_length %u is smaller than the %u special tokens of the template", sp->max_length, n_special);
-  P.budget = sp->max_length ? sp->max_length - n_special : DENSE_NO_LIMIT;
   P.strategy = (uint32_t)sp->strategy;
   P.pad_id = sp->pad_id; P.pad_type = sp->pad_type_id;
   P.trunc_left = sp->truncate_left ? 1 : 0; P.pad_left = sp->pad_left ? 1 : 0;
   dq->docs_per_row = 2;
-  dq->batch_longest = sp->length == 0;
-  dq->multiple = sp->pad_to_multiple_of;
-  P.L = dq->batch_longest ? 0u : dense_round(sp->length, dq->multiple);
-  dq->want_mask = sp->want_mask != 0;
-  return B2T_OK;
+  return dense_length(sp, P.n_pre + P.n_mid + P.n_post, &P.budget, dq);
 }
 
-template <bool OVER, bool OFFS, bool META = false>
-static void launch_rows(Workspace& ws, uint32_t n_rows, const DenseReq& dq, const DenseOverflow& O, cudaStream_t st, const DenseMeta& M = DenseMeta{}) {
+// output k of the workspace's dense rows, null where the request does not ask for it
+template <class T>
+static T* dense_out(const Workspace& ws, const DenseReq& dq, DenseOut k) { return DENSE_OUT[k].wanted(dq) ? ws.dense[k].as<T>() : nullptr; }
+
+// <OVER>: rows of overflowing parts (O's row fields); <OFFS>: offset rows (O's offset fields); <META>: row metadata (M)
+template <bool OVER, bool OFFS, bool META>
+static void launch_rows(Workspace& ws, uint32_t n_rows, const DenseReq& dq, const DenseOverflow& O, const DenseMeta& M, cudaStream_t st) {
   const unsigned grid = (unsigned)(((uint64_t)n_rows * 32 + 255) / 256);
   if (dq.pairs())
-    dense_pair_rows_kernel<OVER, OFFS, META><<<grid, 256, 0, st>>>(ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.P, ws.dense_ids.as<uint32_t>(),
-                                                                   ws.dense_type.as<uint8_t>(), dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr,
-                                                                   ws.dense_len.as<uint32_t>(), O, M);
+    dense_pair_rows_kernel<OVER, OFFS, META><<<grid, 256, 0, st>>>(ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.P, dense_out<uint32_t>(ws, dq, OUT_IDS),
+                                                                   dense_out<uint8_t>(ws, dq, OUT_TYPE), dense_out<uint8_t>(ws, dq, OUT_MASK),
+                                                                   dense_out<uint32_t>(ws, dq, OUT_LEN), O, M);
   else
-    dense_rows_kernel<OVER, OFFS, META><<<grid, 256, 0, st>>>(ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.S, ws.dense_ids.as<uint32_t>(),
-                                                              dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr, ws.dense_len.as<uint32_t>(), nullptr, O, M);
+    dense_rows_kernel<OVER, OFFS, META><<<grid, 256, 0, st>>>(ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.S, dense_out<uint32_t>(ws, dq, OUT_IDS),
+                                                              dense_out<uint8_t>(ws, dq, OUT_MASK), dense_out<uint32_t>(ws, dq, OUT_LEN), nullptr, O, M);
 }
+using LaunchRows = void (*)(Workspace&, uint32_t, const DenseReq&, const DenseOverflow&, const DenseMeta&, cudaStream_t);
+constexpr LaunchRows LAUNCH_ROWS[2][2][2] = {   // [OVER][OFFS][META]
+    {{launch_rows<false, false, false>, launch_rows<false, false, true>}, {launch_rows<false, true, false>, launch_rows<false, true, true>}},
+    {{launch_rows<true, false, false>, launch_rows<true, false, true>}, {launch_rows<true, true, false>, launch_rows<true, true, true>}}};
 
-// The row metadata buffers of n_rows rows and what the META row kernels read (ensures the buffers)
-static int make_meta(b2t_engine* e, Workspace& ws, size_t cells, const DenseReq& dq, DenseMeta* M) {
-  int rc;
-  if ((dq.special_mask && (rc = ws.dense_special.ensure(cells + 16))) || (dq.seq_ids && (rc = ws.dense_seq.ensure(cells + 16))) ||
-      (dq.word_ids && (rc = ws.dense_word.ensure(cells * 4 + 16))))
-    return rc;
-  *M = DenseMeta{dq.trim ? e->d_trim_vocab.as<uint32_t>() : nullptr, e->has_added ? e->d_trim_added.as<AddedTrim>() : nullptr,
-                 e->has_added ? e->n_trim_added : 0u, dq.aps ? 1u : 0u, dq.word_ids ? ws.word_ids.as<uint32_t>() : nullptr,
-                 dq.special_mask ? ws.dense_special.as<uint8_t>() : nullptr, dq.seq_ids ? ws.dense_seq.as<int8_t>() : nullptr,
-                 dq.word_ids ? ws.dense_word.as<uint32_t>() : nullptr, &ws.ctl.as<ctl_block>()->err};
-  return B2T_OK;
-}
-
-// CSR of the workspace -> dense rows in ws.dense_* (asynchronous on st).  n_inputs = documents / docs_per_row; n_rows =
-// n_inputs, or with overflowing parts the rows the count pass found (the host has read them), whose row_sample entries
+// CSR of the workspace -> dense rows in ws.dense (asynchronous on st).  n_inputs = documents / docs_per_row; n_rows =
+// n_inputs, or with overflowing parts the rows the count pass found (the host has read them), whose row sample entries
 // are the inputs' indices + sample_base.
 static int launch_dense(b2t_engine* e, Workspace& ws, uint32_t n_inputs, uint32_t n_rows, const DenseReq& dq, cudaStream_t st, uint32_t sample_base = 0) {
   int rc;
-  const size_t cells = (size_t)n_rows * dq.L();
-  if ((rc = ws.dense_ids.ensure(cells * 4 + 16)) || (rc = ws.dense_len.ensure((size_t)n_rows * 4 + 16)) ||
-      (dq.want_mask && (rc = ws.dense_mask.ensure(cells + 16))) || (dq.pairs() && (rc = ws.dense_type.ensure(cells + 16))))
-    return rc;
+  for (int k = 0; k < N_DENSE_OUT; ++k)
+    if (DENSE_OUT[k].wanted(dq) && (rc = ws.dense[k].ensure(n_rows * dense_row_bytes(k, dq.L()) + 16))) return rc;
+  DenseOverflow O{};
   if (dq.overflow) {
-    if ((rc = ws.row_base.ensure((size_t)n_inputs * 4 + 16)) || (rc = ws.row_sample.ensure((size_t)n_rows * 4 + 16)) ||
-        (dq.offsets && (rc = ws.dense_off.ensure(cells * 8 + 16))))
-      return rc;
+    if ((rc = ws.row_base.ensure((size_t)n_inputs * 4 + 16))) return rc;
     if (n_inputs)
       dense_row_sample_kernel<<<(unsigned)(((uint64_t)n_inputs * 32 + 255) / 256), 256, 0, st>>>(
           ws.row_count.as<uint32_t>(), ws.row_lexcl.as<unsigned long long>(), ws.row_bsum.as<unsigned long long>(), TSCAN, n_inputs, sample_base,
-          ws.row_base.as<uint32_t>(), ws.row_sample.as<uint32_t>());
+          ws.row_base.as<uint32_t>(), ws.dense[OUT_SAMPLE].as<uint32_t>());
     e->last_launches++;
     rec(e, st, "dense_row_sample");   // (from the end of dense_count: includes the host's read of the row count)
     const bool b_first = dq.pairs() && dq.P.b_first;
-    DenseOverflow O{ws.row_sample.as<uint32_t>(), ws.row_base.as<uint32_t>(), sample_base, dq.stride,
-                    b_first ? dq.type_ob : dq.type_oa, b_first ? dq.type_oa : dq.type_ob,
-                    dq.offsets ? ws.offsets.as<uint2>() : nullptr, dq.offsets ? ws.dense_off.as<uint2>() : nullptr};
-    DenseMeta M{};
-    if (dq.meta() && (rc = make_meta(e, ws, cells, dq, &M))) return rc;
-    if (n_rows && dq.L()) {
-      if (dq.meta() && dq.offsets) launch_rows<true, true, true>(ws, n_rows, dq, O, st, M);
-      else if (dq.meta()) launch_rows<true, false, true>(ws, n_rows, dq, O, st, M);
-      else if (dq.offsets) launch_rows<true, true>(ws, n_rows, dq, O, st);
-      else launch_rows<true, false>(ws, n_rows, dq, O, st);
-    }
-    e->last_launches++;
-    rec(e, st, dq.pairs() ? "dense_pair_rows_overflow" : "dense_rows_overflow");
-    CU(cudaGetLastError());
-    return B2T_OK;
+    O.row_sample = ws.dense[OUT_SAMPLE].as<uint32_t>(); O.row_base = ws.row_base.as<uint32_t>(); O.sample_base = sample_base; O.stride = dq.stride;
+    O.type_ox = b_first ? dq.type_ob : dq.type_oa; O.type_oy = b_first ? dq.type_oa : dq.type_ob;
   }
-  if (dq.offsets || dq.meta()) {   // offset rows of the kept parts only (the <0, 1> instantiations) and / or row metadata (<0, *, 1>)
-    if (dq.offsets && (rc = ws.dense_off.ensure(cells * 8 + 16))) return rc;
-    DenseOverflow O{};
-    if (dq.offsets) O = DenseOverflow{nullptr, nullptr, 0u, 0u, 0u, 0u, ws.offsets.as<uint2>(), ws.dense_off.as<uint2>()};
-    DenseMeta M{};
-    if (dq.meta() && (rc = make_meta(e, ws, cells, dq, &M))) return rc;
-    if (n_rows && dq.L()) {
-      if (dq.meta() && dq.offsets) launch_rows<false, true, true>(ws, n_rows, dq, O, st, M);
-      else if (dq.meta()) launch_rows<false, false, true>(ws, n_rows, dq, O, st, M);
-      else launch_rows<false, true>(ws, n_rows, dq, O, st);
-    }
-    e->last_launches++;
-    CU(cudaGetLastError());
-    return B2T_OK;
-  }
-  const unsigned grid = (unsigned)(((uint64_t)n_rows * 32 + 255) / 256);
-  if (n_rows && dq.L() && dq.pairs())
-    dense_pair_rows_kernel<<<grid, 256, 0, st>>>(ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.P, ws.dense_ids.as<uint32_t>(),
-                                                 ws.dense_type.as<uint8_t>(), dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr,
-                                                 ws.dense_len.as<uint32_t>());
-  else if (n_rows && dq.L())
-    dense_rows_kernel<<<grid, 256, 0, st>>>(
-        ws.ids.as<uint32_t>(), ws.row_ptr.as<uint64_t>(), n_rows, dq.S, ws.dense_ids.as<uint32_t>(),
-        dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr, ws.dense_len.as<uint32_t>(), nullptr);
+  if (dq.offsets) { O.offsets = ws.offsets.as<uint2>(); O.out_off = ws.dense[OUT_OFF].as<uint2>(); }
+  DenseMeta M{};
+  if (dq.meta())
+    M = DenseMeta{dq.trim ? e->d_trim_vocab.as<uint32_t>() : nullptr, e->has_added ? e->d_trim_added.as<AddedTrim>() : nullptr,
+                  e->has_added ? e->n_trim_added : 0u, dq.aps ? 1u : 0u, dq.word_ids ? ws.word_ids.as<uint32_t>() : nullptr,
+                  dense_out<uint8_t>(ws, dq, OUT_SPECIAL), dense_out<int8_t>(ws, dq, OUT_SEQ), dense_out<uint32_t>(ws, dq, OUT_WORD),
+                  &ws.ctl.as<ctl_block>()->err};
+  if (n_rows && dq.L()) LAUNCH_ROWS[dq.overflow][dq.offsets][dq.meta()](ws, n_rows, dq, O, M, st);
   e->last_launches++;
+  if (dq.overflow) rec(e, st, dq.pairs() ? "dense_pair_rows_overflow" : "dense_rows_overflow");
   CU(cudaGetLastError());
   return B2T_OK;
 }
@@ -1041,10 +1031,10 @@ extern "C" int b2t_encode_batch_device(b2t_engine* e, const uint8_t* d_bytes, ui
     b2t_result* r = new b2t_result();
     r->eng = e; r->on_device = 1; r->n_docs = n_docs;
     r->n_tokens = ws.h_ctl.as<ctl_block>()->total;
-    r->ids = ws.ids.as<uint32_t>();
-    r->offsets = (flags & B2T_WANT_OFFSETS) ? ws.offsets.as<uint32_t>() : nullptr;
-    r->word_ids = (flags & B2T_WANT_WORD_IDS) ? ws.word_ids.as<uint32_t>() : nullptr;
-    r->row_ptr = ws.row_ptr.as<uint64_t>();
+    r->view.ids = ws.ids.as<uint32_t>();
+    r->view.offsets = (flags & B2T_WANT_OFFSETS) ? ws.offsets.as<uint32_t>() : nullptr;
+    r->view.word_ids = (flags & B2T_WANT_WORD_IDS) ? ws.word_ids.as<uint32_t>() : nullptr;
+    r->view.row_ptr = ws.row_ptr.as<uint64_t>();
     *out = r;
     return B2T_OK;
   });
@@ -1165,38 +1155,42 @@ static int overflow_rows(const ctl_block* c, uint64_t before, uint32_t L, uint32
   return B2T_OK;
 }
 
-extern "C" int b2t_encode_batch_dense(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs, const b2t_dense_spec* spec,
-                                      b2t_result** out);
+// After the host has read the control block of a dense run of n_in inputs: L under BatchLongest, or the check that every
+// row fits a fixed L; with overflowing parts the rows the run makes (`before` rows of the result precede them, the
+// first input is sample_base); then the row kernels that had to wait for either (a fixed L without overflowing parts:
+// queued with the run), asynchronous on st.  `room(*n_rows)` runs before they are queued: the host path makes room for
+// the rows in its pinned result there.
+template <class Room>
+static int dense_after_count(b2t_engine* e, Workspace& ws, DenseReq& dq, uint32_t n_in, uint64_t before, uint32_t sample_base, cudaStream_t st,
+                             uint32_t* n_rows, Room&& room) {
+  const ctl_block* c = ws.h_ctl.as<ctl_block>();
+  int rc;
+  if (dq.batch_longest) dq.L() = dense_round(c->max_row, dq.multiple);
+  else if (c->max_row > dq.L())
+    return fail(B2T_ERR_INVALID, "a row of %u tokens does not fit the dense length %u: enable truncation (the reference returns a longer row here)", c->max_row, dq.L());
+  *n_rows = n_in;
+  if (dq.overflow && (rc = overflow_rows(c, before, dq.L(), n_rows))) return rc;
+  if ((rc = room(*n_rows))) return rc;
+  if ((dq.batch_longest || dq.overflow) && ((rc = launch_dense(e, ws, n_in, *n_rows, dq, st, sample_base)) || (rc = meta_check(e, ws, dq, st)))) return rc;
+  return B2T_OK;
+}
 
-// the dense device entry points: the rows of n_rows rows (n_docs / dq.docs_per_row) after the run
+// the dense device entry points: the rows of n_docs / dq.docs_per_row inputs after the run, asynchronous on the stream
+// like the CSR entry point's result
 template <class Spec>
 static int dense_device(const char* fn, b2t_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint64_t* d_doc_off, uint32_t n_docs,
                         const Spec* spec, void* stream, b2t_result** out) {
   DenseReq dq;
   return device_encode(fn, e, out, d_bytes, n_bytes, d_doc_off, n_docs, 0u, RUN_RESULT, spec, &dq, stream,
                        [&](Workspace& ws, cudaStream_t st) -> int {
-    int rc2;
-    const ctl_block* c = ws.h_ctl.as<ctl_block>();
-    const uint32_t max_row = c->max_row, n_in = n_docs / dq.docs_per_row;
-    uint32_t n_rows = n_in;
-    if (dq.batch_longest) dq.L() = dense_round(max_row, dq.multiple);
-    else if (max_row > dq.L())
-      return fail(B2T_ERR_INVALID, "a row of %u tokens does not fit the dense length %u: enable truncation (the reference returns a longer row here)", max_row, dq.L());
-    if (dq.overflow && (rc2 = overflow_rows(c, 0, dq.L(), &n_rows))) return rc2;
-    // asynchronous on st, like the CSR entry point's result (a fixed length without overflowing parts: queued already)
-    if ((dq.batch_longest || dq.overflow) && ((rc2 = launch_dense(e, ws, n_in, n_rows, dq, st)) || (rc2 = meta_check(e, ws, dq, st)))) return rc2;
+    const uint32_t n_in = n_docs / dq.docs_per_row;
+    uint32_t n_rows = 0;
+    int rc2 = dense_after_count(e, ws, dq, n_in, 0, 0, st, &n_rows, [](uint32_t) { return B2T_OK; });
+    if (rc2) return rc2;
     b2t_result* r = new b2t_result();
-    r->eng = e; r->on_device = 1; r->n_docs = n_in; r->n_rows = n_rows;
-    r->row_sample = dq.overflow ? ws.row_sample.as<uint32_t>() : nullptr;
-    r->dense_off = dq.offsets ? ws.dense_off.as<uint32_t>() : nullptr;
+    r->eng = e; r->on_device = 1; r->n_docs = n_in;
     r->n_tokens = ws.h_ctl.as<ctl_block>()->total;
-    r->dense_len = dq.L();
-    r->dense_ids = ws.dense_ids.as<uint32_t>(); r->row_len = ws.dense_len.as<uint32_t>();
-    r->dense_mask = dq.want_mask ? ws.dense_mask.as<uint8_t>() : nullptr;
-    r->type_ids = dq.pairs() ? ws.dense_type.as<uint8_t>() : nullptr;
-    r->special_mask = dq.special_mask ? ws.dense_special.as<uint8_t>() : nullptr;
-    r->seq_ids = dq.seq_ids ? ws.dense_seq.as<int8_t>() : nullptr;
-    r->dense_word = dq.word_ids ? ws.dense_word.as<uint32_t>() : nullptr;
+    set_dense_views(r, dq, n_rows, ws.dense);
     *out = r;
     return B2T_OK;
   });
@@ -1227,8 +1221,7 @@ static b2t_result* pool_get(b2t_engine* e) {
   std::lock_guard<std::mutex> lk(e->mu);
   if (!e->pool.empty()) {
     b2t_result* r = e->pool.back().release(); e->pool.pop_back();
-    r->type_ids = nullptr; r->n_rows = 0; r->row_sample = nullptr; r->dense_off = nullptr;
-    r->special_mask = nullptr; r->seq_ids = nullptr; r->dense_word = nullptr;
+    r->view = {};
     return r;
   }
   return new b2t_result();
@@ -1274,18 +1267,11 @@ struct Chunk { uint32_t d0, d1; uint64_t b0, b1; uint64_t tok_base; };
 
 // Queues the copy of a chunk's dense rows (rows r0 .. r0 + nr - 1) into the pinned result, on the slot's stream.
 static int queue_dense_copy(b2t_result* r, const Workspace& ws, uint32_t r0, uint32_t nr, const DenseReq& dq) {
-  const size_t L = dq.L();
-  if (nr && L) {
-    CU(cudaMemcpyAsync(r->h_dense_ids.as<uint32_t>() + (size_t)r0 * L, ws.dense_ids.p, (size_t)nr * L * 4, cudaMemcpyDeviceToHost, ws.stream));
-    if (dq.want_mask) CU(cudaMemcpyAsync(r->h_dense_mask.as<uint8_t>() + (size_t)r0 * L, ws.dense_mask.p, (size_t)nr * L, cudaMemcpyDeviceToHost, ws.stream));
-    if (dq.pairs()) CU(cudaMemcpyAsync(r->h_type_ids.as<uint8_t>() + (size_t)r0 * L, ws.dense_type.p, (size_t)nr * L, cudaMemcpyDeviceToHost, ws.stream));
-    if (dq.offsets) CU(cudaMemcpyAsync(r->h_dense_off.as<uint32_t>() + (size_t)r0 * L * 2, ws.dense_off.p, (size_t)nr * L * 8, cudaMemcpyDeviceToHost, ws.stream));
-    if (dq.special_mask) CU(cudaMemcpyAsync(r->h_special.as<uint8_t>() + (size_t)r0 * L, ws.dense_special.p, (size_t)nr * L, cudaMemcpyDeviceToHost, ws.stream));
-    if (dq.seq_ids) CU(cudaMemcpyAsync(r->h_seq.as<int8_t>() + (size_t)r0 * L, ws.dense_seq.p, (size_t)nr * L, cudaMemcpyDeviceToHost, ws.stream));
-    if (dq.word_ids) CU(cudaMemcpyAsync(r->h_word.as<uint32_t>() + (size_t)r0 * L, ws.dense_word.p, (size_t)nr * L * 4, cudaMemcpyDeviceToHost, ws.stream));
+  for (int k = 0; k < N_DENSE_OUT; ++k) {
+    const size_t row = dense_row_bytes(k, dq.L());
+    if (DENSE_OUT[k].wanted(dq) && nr && row)
+      CU(cudaMemcpyAsync(r->h_dense[k].as<uint8_t>() + r0 * row, ws.dense[k].p, nr * row, cudaMemcpyDeviceToHost, ws.stream));
   }
-  if (nr) CU(cudaMemcpyAsync(r->h_row_len.as<uint32_t>() + r0, ws.dense_len.p, (size_t)nr * 4, cudaMemcpyDeviceToHost, ws.stream));
-  if (nr && dq.overflow) CU(cudaMemcpyAsync(r->h_row_sample.as<uint32_t>() + r0, ws.row_sample.p, (size_t)nr * 4, cudaMemcpyDeviceToHost, ws.stream));
   return B2T_OK;
 }
 
@@ -1332,23 +1318,16 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     if (want_wid && (rc2 = r->h_word_ids.ensure(need_tok * 4, true))) return rc2;
     return B2T_OK;
   };
-  r->dense_len = 0; r->dense_ids = nullptr; r->dense_mask = nullptr; r->row_len = nullptr; r->type_ids = nullptr;
-  r->special_mask = nullptr; r->seq_ids = nullptr; r->dense_word = nullptr;
   // pinned rows: the whole batch's n_rows rows, or with overflowing parts a guess grown on demand (contents kept)
   uint64_t cap_rows = 0, row_total = 0;
-  auto dense_host = [&](uint32_t L, uint64_t rows, bool keep) -> int {
+  auto dense_host = [&](uint64_t rows, bool keep) -> int {
     int rc2;
-    const size_t cells = (size_t)rows * L;
-    if ((rc2 = r->h_dense_ids.ensure(cells * 4 + 16, keep)) || (rc2 = r->h_row_len.ensure((size_t)rows * 4 + 16, keep)) ||
-        (dq->want_mask && (rc2 = r->h_dense_mask.ensure(cells + 16, keep))) || (dq->pairs() && (rc2 = r->h_type_ids.ensure(cells + 16, keep))) ||
-        (dq->overflow && (rc2 = r->h_row_sample.ensure((size_t)rows * 4 + 16, keep))) || (dq->offsets && (rc2 = r->h_dense_off.ensure(cells * 8 + 16, keep))) ||
-        (dq->special_mask && (rc2 = r->h_special.ensure(cells + 16, keep))) || (dq->seq_ids && (rc2 = r->h_seq.ensure(cells + 16, keep))) ||
-        (dq->word_ids && (rc2 = r->h_word.ensure(cells * 4 + 16, keep))))
-      return rc2;
+    for (int k = 0; k < N_DENSE_OUT; ++k)
+      if (DENSE_OUT[k].wanted(*dq) && (rc2 = r->h_dense[k].ensure(rows * dense_row_bytes(k, dq->L()) + 16, keep))) return rc2;
     cap_rows = rows;
     return B2T_OK;
   };
-  if (dq) { if (!dq->batch_longest && (rc = dense_host(dq->L(), n_rows, false))) { pool_put(e, r); return rc; } }
+  if (dq) { if (!dq->batch_longest && (rc = dense_host(n_rows, false))) { pool_put(e, r); return rc; } }
   else if ((rc = grow(cap_tok))) { pool_put(e, r); return rc; }
 
   uint64_t tok_base = 0;
@@ -1366,26 +1345,17 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
     const uint64_t nt = ws.h_ctl.as<ctl_block>()->total;
     c.tok_base = tok_base;
     if (dq) {
-      const ctl_block* cb = ws.h_ctl.as<ctl_block>();
-      const uint32_t n_in = (c.d1 - c.d0) / per, max_row = cb->max_row;
-      uint32_t nr = n_in;
-      if (dq->batch_longest) {   // one chunk: L is known now
-        dq->L() = dense_round(max_row, dq->multiple);
-        if (!dq->overflow && (rc2 = dense_host(dq->L(), n_rows, false))) return rc2;
-      } else if (max_row > dq->L()) {
-        return fail(B2T_ERR_INVALID, "a row of %u tokens does not fit the dense length %u: enable truncation (the reference returns a longer row here)", max_row, dq->L());
-      }
-      if (dq->overflow) {
-        // the chunk's rows go at the running row base; earlier chunks may still be copying into the old buffers: let them
-        // land, then grow (contents are kept)
-        if ((rc2 = overflow_rows(cb, row_total, dq->L(), &nr))) return rc2;
-        if (row_total + nr > cap_rows) {
+      uint32_t nr = 0;
+      auto room = [&](uint32_t rows) -> int {
+        if (dq->overflow && row_total + rows > cap_rows) {
+          // the chunk's rows go at the running row base; earlier chunks may still be copying into the old buffers: let
+          // them land, then grow (contents are kept)
           for (auto& s : ss.slot) if (s.stream) CU(cudaStreamSynchronize(s.stream));
-          if ((rc2 = dense_host(dq->L(), std::max<uint64_t>((row_total + nr) * 2, (uint64_t)n_rows), true))) return rc2;
+          return dense_host(std::max<uint64_t>((row_total + rows) * 2, (uint64_t)n_rows), true);
         }
-      }
-      if ((dq->batch_longest || dq->overflow) && ((rc2 = launch_dense(e, ws, n_in, nr, *dq, ws.stream, c.d0 / per)) || (rc2 = meta_check(e, ws, *dq, ws.stream))))
-        return rc2;
+        return (dq->batch_longest && !dq->overflow) ? dense_host(n_rows, false) : B2T_OK;   // (one chunk: L is known now)
+      };
+      if ((rc2 = dense_after_count(e, ws, *dq, (c.d1 - c.d0) / per, row_total, c.d0 / per, ws.stream, &nr, room))) return rc2;
       // (a fixed length without overflowing parts: the rows were queued for the copy right behind the kernels, see issue();
       // a rerun has replaced them)
       if ((dq->batch_longest || dq->overflow || reran) && (rc2 = queue_dense_copy(r, ws, (uint32_t)row_total, nr, *dq))) return rc2;
@@ -1448,17 +1418,8 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
 
   if (dq) {
     if (n_docs == 0 && dq->batch_longest) dq->L() = 0;
-    r->n_tokens = tok_base; r->ids = nullptr; r->offsets = nullptr; r->word_ids = nullptr; r->row_ptr = nullptr;
-    r->dense_len = dq->L();
-    r->dense_ids = r->h_dense_ids.as<uint32_t>(); r->row_len = r->h_row_len.as<uint32_t>();
-    r->dense_mask = dq->want_mask ? r->h_dense_mask.as<uint8_t>() : nullptr;
-    r->type_ids = dq->pairs() ? r->h_type_ids.as<uint8_t>() : nullptr;
-    r->n_rows = (uint32_t)row_total;
-    r->row_sample = dq->overflow ? r->h_row_sample.as<uint32_t>() : nullptr;
-    r->dense_off = dq->offsets ? r->h_dense_off.as<uint32_t>() : nullptr;
-    r->special_mask = dq->special_mask ? r->h_special.as<uint8_t>() : nullptr;
-    r->seq_ids = dq->seq_ids ? r->h_seq.as<int8_t>() : nullptr;
-    r->dense_word = dq->word_ids ? r->h_word.as<uint32_t>() : nullptr;
+    r->n_tokens = tok_base;
+    set_dense_views(r, *dq, (uint32_t)row_total, r->h_dense);
   } else {
     // chunk-relative row_ptr -> batch-relative (host fix-up: one addition per document)
     uint64_t* rp = r->h_row_ptr.as<uint64_t>();
@@ -1468,10 +1429,10 @@ static int host_encode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* by
       for (uint32_t d = c.d0; d <= hi; ++d) rp[d] += c.tok_base;
     }
     r->n_tokens = tok_base;
-    r->ids = r->h_ids.as<uint32_t>();
-    r->offsets = want_off ? r->h_offsets.as<uint32_t>() : nullptr;
-    r->word_ids = want_wid ? r->h_word_ids.as<uint32_t>() : nullptr;
-    r->row_ptr = rp;
+    r->view.ids = r->h_ids.as<uint32_t>();
+    r->view.offsets = want_off ? r->h_offsets.as<uint32_t>() : nullptr;
+    r->view.word_ids = want_wid ? r->h_word_ids.as<uint32_t>() : nullptr;
+    r->view.row_ptr = rp;
   }
   *out = r;
   return B2T_OK;
@@ -1579,7 +1540,7 @@ static int pre_tokenize(b2t_engine* e, b2t_engine::SlotSet& ss, const uint8_t* b
   if ((rc = r->h_offsets.ensure((k + 1) * 8, false))) { pool_put(e, r); return rc; }
   uint32_t* off = r->h_offsets.as<uint32_t>();
   if (k) memcpy(off, pairs.data(), k * 8);
-  r->n_tokens = k; r->ids = nullptr; r->word_ids = nullptr; r->offsets = off; r->row_ptr = rp;
+  r->n_tokens = k; r->view.offsets = off; r->view.row_ptr = rp;
   *out = r;
   return B2T_OK;
 }
@@ -1593,21 +1554,23 @@ extern "C" int b2t_pre_tokenize_batch(b2t_engine* e, const uint8_t* bytes, const
 extern "C" uint64_t b2t_result_n_tokens(const b2t_result* r) { return r ? r->n_tokens : 0; }
 extern "C" uint32_t b2t_result_n_docs(const b2t_result* r) { return r ? r->n_docs : 0; }
 extern "C" int b2t_result_on_device(const b2t_result* r) { return r ? r->on_device : 0; }
-extern "C" const uint32_t* b2t_result_ids(const b2t_result* r) { return r ? r->ids : nullptr; }
-extern "C" const uint32_t* b2t_result_offsets(const b2t_result* r) { return r ? r->offsets : nullptr; }
-extern "C" const uint32_t* b2t_result_word_ids(const b2t_result* r) { return r ? r->word_ids : nullptr; }
-extern "C" const uint64_t* b2t_result_row_ptr(const b2t_result* r) { return r ? r->row_ptr : nullptr; }
-extern "C" uint32_t b2t_result_dense_length(const b2t_result* r) { return r ? r->dense_len : 0; }
-extern "C" const uint32_t* b2t_result_dense_ids(const b2t_result* r) { return r ? r->dense_ids : nullptr; }
-extern "C" const uint8_t* b2t_result_attention_mask(const b2t_result* r) { return r ? r->dense_mask : nullptr; }
-extern "C" const uint32_t* b2t_result_row_lengths(const b2t_result* r) { return r ? r->row_len : nullptr; }
-extern "C" const uint8_t* b2t_result_type_ids(const b2t_result* r) { return r ? r->type_ids : nullptr; }
-extern "C" uint32_t b2t_result_dense_rows(const b2t_result* r) { return r ? r->n_rows : 0; }
-extern "C" const uint32_t* b2t_result_row_sample(const b2t_result* r) { return r ? r->row_sample : nullptr; }
-extern "C" const uint32_t* b2t_result_dense_offsets(const b2t_result* r) { return r ? r->dense_off : nullptr; }
-extern "C" const uint8_t* b2t_result_special_tokens_mask(const b2t_result* r) { return r ? r->special_mask : nullptr; }
-extern "C" const int8_t* b2t_result_sequence_ids(const b2t_result* r) { return r ? r->seq_ids : nullptr; }
-extern "C" const uint32_t* b2t_result_dense_word_ids(const b2t_result* r) { return r ? r->dense_word : nullptr; }
+extern "C" const uint32_t* b2t_result_ids(const b2t_result* r) { return r ? r->view.ids : nullptr; }
+extern "C" const uint32_t* b2t_result_offsets(const b2t_result* r) { return r ? r->view.offsets : nullptr; }
+extern "C" const uint32_t* b2t_result_word_ids(const b2t_result* r) { return r ? r->view.word_ids : nullptr; }
+extern "C" const uint64_t* b2t_result_row_ptr(const b2t_result* r) { return r ? r->view.row_ptr : nullptr; }
+extern "C" uint32_t b2t_result_dense_length(const b2t_result* r) { return r ? r->view.dense_len : 0; }
+extern "C" uint32_t b2t_result_dense_rows(const b2t_result* r) { return r ? r->view.n_rows : 0; }
+template <class T>
+static const T* dense_view(const b2t_result* r, DenseOut k) { return r ? static_cast<const T*>(r->view.dense[k]) : nullptr; }
+extern "C" const uint32_t* b2t_result_dense_ids(const b2t_result* r) { return dense_view<uint32_t>(r, OUT_IDS); }
+extern "C" const uint8_t* b2t_result_attention_mask(const b2t_result* r) { return dense_view<uint8_t>(r, OUT_MASK); }
+extern "C" const uint32_t* b2t_result_row_lengths(const b2t_result* r) { return dense_view<uint32_t>(r, OUT_LEN); }
+extern "C" const uint8_t* b2t_result_type_ids(const b2t_result* r) { return dense_view<uint8_t>(r, OUT_TYPE); }
+extern "C" const uint32_t* b2t_result_row_sample(const b2t_result* r) { return dense_view<uint32_t>(r, OUT_SAMPLE); }
+extern "C" const uint32_t* b2t_result_dense_offsets(const b2t_result* r) { return dense_view<uint32_t>(r, OUT_OFF); }
+extern "C" const uint8_t* b2t_result_special_tokens_mask(const b2t_result* r) { return dense_view<uint8_t>(r, OUT_SPECIAL); }
+extern "C" const int8_t* b2t_result_sequence_ids(const b2t_result* r) { return dense_view<int8_t>(r, OUT_SEQ); }
+extern "C" const uint32_t* b2t_result_dense_word_ids(const b2t_result* r) { return dense_view<uint32_t>(r, OUT_WORD); }
 extern "C" void b2t_result_free(b2t_result* r) {
   if (!r) return;
   if (r->on_device || !r->eng) { delete r; return; }

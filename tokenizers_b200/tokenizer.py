@@ -886,44 +886,37 @@ class Tokenizer:
         sp.n_pieces, sp.piece_ids, sp.piece_types = len(pieces), keep[0].ctypes.data, keep[1].ctypes.data
         return sp, keep
 
-    def _dense_call(self, entry, data, doc_off, n_rows, sp, want_mask, type_ids):
-        """b2t_encode_batch_dense / b2t_encode_pairs_dense -> (ids [R, L], mask [R, L] | None, lengths [R], type ids [R, L] | None,
-        row sample [R] | None, offsets [R, L, 2] | None, special-tokens mask [R, L] | None, sequence ids [R, L] | None, word ids
-        [R, L] | None); R = n_rows without overflowing parts"""
+    # The outputs of a dense call in the order of its dict: key, accessor, dtype, what a row holds ("pos": a value per
+    # position, "pos2": a pair per position, "row": one value) and whether the spec asks for it.
+    _DENSE_OUTPUTS = (
+        ("input_ids", "b2t_result_dense_ids", np.uint32, "pos", lambda sp: True),
+        ("token_type_ids", "b2t_result_type_ids", np.uint8, "pos", lambda sp: isinstance(sp, _lib.PairDenseSpec)),
+        ("attention_mask", "b2t_result_attention_mask", np.uint8, "pos", lambda sp: sp.want_mask),
+        ("lengths", "b2t_result_row_lengths", np.uint32, "row", lambda sp: True),
+        ("overflow_to_sample_mapping", "b2t_result_row_sample", np.uint32, "row", lambda sp: sp.dense_flags & _lib.DENSE_OVERFLOW),
+        ("offset_mapping", "b2t_result_dense_offsets", np.uint32, "pos2", lambda sp: sp.dense_flags & _lib.DENSE_OFFSETS),
+        ("special_tokens_mask", "b2t_result_special_tokens_mask", np.uint8, "pos", lambda sp: sp.dense_flags & _lib.DENSE_SPECIAL_MASK),
+        ("sequence_ids", "b2t_result_sequence_ids", np.int8, "pos", lambda sp: sp.dense_flags & _lib.DENSE_SEQUENCE_IDS),
+        ("word_ids", "b2t_result_dense_word_ids", np.int32, "pos", lambda sp: sp.dense_flags & _lib.DENSE_WORD_IDS),   # -1 = None
+    )
+
+    def _dense_call(self, entry, data, doc_off, n_rows, sp):
+        """b2t_encode_batch_dense / b2t_encode_pairs_dense -> {key: rows} of the outputs sp asks for, and "attention_mask":
+        None without a mask; [R, L] per position ([R, L, 2] offsets) or [R] per row, R = n_rows without overflowing parts"""
         if self._added is not None and not self._dev_added and added.split_batch(self._added, data, doc_off)[2]:
             raise UnsupportedConfig("the batch contains added tokens and this configuration extracts them on the host: use encode_batch")
         L = _lib.lib()
         res = ctypes.c_void_p()
         _lib.check(getattr(L, entry)(self._h, data.ctypes.data if data.size else None, doc_off.ctypes.data, n_rows, ctypes.byref(sp), ctypes.byref(res)))
+        asked = [want(sp) for *_, want in self._DENSE_OUTPUTS]
 
         def views(L, res):
             W, R = L.b2t_result_dense_length(res), L.b2t_result_dense_rows(res)
-            return (_view(L.b2t_result_dense_ids(res), R * W, np.uint32).reshape(R, W),
-                    _view(L.b2t_result_attention_mask(res), R * W, np.uint8).reshape(R, W) if want_mask else None,
-                    _view(L.b2t_result_row_lengths(res), R, np.uint32),
-                    _view(L.b2t_result_type_ids(res), R * W, np.uint8).reshape(R, W) if type_ids else None,
-                    _view(L.b2t_result_row_sample(res), R, np.uint32) if sp.dense_flags & _lib.DENSE_OVERFLOW else None,
-                    _view(L.b2t_result_dense_offsets(res), 2 * R * W, np.uint32).reshape(R, W, 2) if sp.dense_flags & _lib.DENSE_OFFSETS else None,
-                    _view(L.b2t_result_special_tokens_mask(res), R * W, np.uint8).reshape(R, W) if sp.dense_flags & _lib.DENSE_SPECIAL_MASK else None,
-                    _view(L.b2t_result_sequence_ids(res), R * W, np.int8).reshape(R, W) if sp.dense_flags & _lib.DENSE_SEQUENCE_IDS else None,
-                    _view(L.b2t_result_dense_word_ids(res), R * W, np.uint32).reshape(R, W) if sp.dense_flags & _lib.DENSE_WORD_IDS else None)
-        return _read_result(self, res, views)[0]
-
-    @staticmethod
-    def _dense_dict(out, rows, overflow, offsets):
-        """the dict of a dense call: rows = what _dense_call returned, plus the optional overflow / offset / metadata entries
-        (word ids as int32 with -1 for None)"""
-        if overflow:
-            out["overflow_to_sample_mapping"] = rows[4]
-        if offsets:
-            out["offset_mapping"] = rows[5]
-        if rows[6] is not None:
-            out["special_tokens_mask"] = rows[6]
-        if rows[7] is not None:
-            out["sequence_ids"] = rows[7]
-        if rows[8] is not None:
-            out["word_ids"] = rows[8].view(np.int32)
-        return out
+            shapes = {"pos": (R, W), "pos2": (R, W, 2), "row": (R,)}
+            return tuple(_view(getattr(L, acc)(res), int(np.prod(shapes[row])), dt).reshape(shapes[row]) if a else None
+                         for (_, acc, dt, row, _), a in zip(self._DENSE_OUTPUTS, asked))
+        rows = _read_result(self, res, views)[0]
+        return {key: v for (key, *_), v, a in zip(self._DENSE_OUTPUTS, rows, asked) if a or key == "attention_mask"}
 
     def encode_batch_dense(self, data, doc_off=None, add_special_tokens=True, want_mask=True, return_overflowing_tokens=False,
                            return_offsets_mapping=False, trim_offsets=False, return_special_tokens_mask=False, return_sequence_ids=False,
@@ -949,15 +942,13 @@ class Tokenizer:
         sp, keep = self.dense_spec(add_special_tokens, want_mask, return_overflowing_tokens, return_offsets_mapping, trim_offsets,
                                    return_special_tokens_mask, return_sequence_ids, return_word_ids)
         try:
-            rows = self._dense_call("b2t_encode_batch_dense", data, doc_off, len(doc_off) - 1, sp, want_mask, False)
+            return self._dense_call("b2t_encode_batch_dense", data, doc_off, len(doc_off) - 1, sp)
         except B2TError as ex:
             if ex.code == _lib.B2T_ERR_TRUNCATION:   # the reference's stride panic, with its message
                 raise ValueError(str(ex)) from None
             if ex.code == _lib.B2T_ERR_UNSUPPORTED and sp.dense_flags & _lib.DENSE_TRIM_OFFSETS:   # (the lstrip + rstrip refusal)
                 raise UnsupportedConfig(str(ex)) from None
             raise
-        return self._dense_dict({"input_ids": rows[0], "attention_mask": rows[1], "lengths": rows[2]}, rows, return_overflowing_tokens,
-                                return_offsets_mapping)
 
     def encode_pairs_dense(self, pairs, doc_off=None, add_special_tokens=True, want_mask=True, return_overflowing_tokens=False,
                            return_offsets_mapping=False, trim_offsets=False, return_special_tokens_mask=False, return_sequence_ids=False,
@@ -985,15 +976,13 @@ class Tokenizer:
         sp, keep = self.pair_dense_spec(add_special_tokens, want_mask, return_overflowing_tokens, return_offsets_mapping, trim_offsets,
                                         return_special_tokens_mask, return_sequence_ids, return_word_ids)
         try:
-            rows = self._dense_call("b2t_encode_pairs_dense", data, doc_off, (len(doc_off) - 1) // 2, sp, want_mask, True)
+            return self._dense_call("b2t_encode_pairs_dense", data, doc_off, (len(doc_off) - 1) // 2, sp)
         except B2TError as ex:
             if ex.code == _lib.B2T_ERR_TRUNCATION:   # TruncationError::SequenceTooShort, with the reference's message
                 raise ValueError(str(ex)) from None
             if ex.code == _lib.B2T_ERR_UNSUPPORTED:
                 raise UnsupportedConfig(str(ex)) from None
             raise
-        return self._dense_dict({"input_ids": rows[0], "token_type_ids": rows[3], "attention_mask": rows[1], "lengths": rows[2]}, rows,
-                                return_overflowing_tokens, return_offsets_mapping)
 
     def _trim_tables(self):
         """per token id: leading / trailing 'G-dot' characters (the byte-level image of U+0020) of its vocabulary string"""
