@@ -366,8 +366,10 @@ extern "C" int b2t_engine_create(const b2t_config* cfg, b2t_engine** out) {
   e->dt.max_chars = ht.max_chars;
   // the page kernels use ~23 KB of shared memory per block, 8 blocks per SM: leave the rest of the 228 KB pool to L1
   // (the merge-table probes of the merge rounds are read-only loads and hit there)
-  cudaFuncSetAttribute(model_tile_kernel<MODEL_BPE>, cudaFuncAttributePreferredSharedMemoryCarveout, 86);
-  cudaFuncSetAttribute(model_tile_kernel<MODEL_WORDPIECE>, cudaFuncAttributePreferredSharedMemoryCarveout, 86);
+  for (int i = 0; i < N_MODEL_LAYOUTS; ++i) {
+    cudaFuncSetAttribute(model_kernel<MODEL_BPE>(i), cudaFuncAttributePreferredSharedMemoryCarveout, 86);
+    cudaFuncSetAttribute(model_kernel<MODEL_WORDPIECE>(i), cudaFuncAttributePreferredSharedMemoryCarveout, 86);
+  }
   if (cfg->model == B2T_MODEL_BPE) {   // (the ByteLevel pre-tokenizers: the only ones BPE runs behind)
     if ((rc = upload(e->d_trim_vocab, vocab_trim_counts(cfg->n_vocab, cfg->vocab_bytes, cfg->vocab_off, cfg->vocab_ids)))) return rc;
     e->trim_ready = 1;
@@ -825,16 +827,22 @@ static void long_pretokens(b2t_engine* e, Workspace& ws, const Batch& b, cudaStr
 }
 
 // K2 model_tile into provisional slots, then pass 2's page token counts -> exclusive scan (the total goes to the control block)
-static void model_and_count(b2t_engine* e, Workspace& ws, const Batch& b, uint32_t flags, bool added, cudaStream_t st) {
+static int model_and_count(b2t_engine* e, Workspace& ws, const Batch& b, uint32_t flags, bool added, cudaStream_t st) {
   const int64_t n_pages = b.n / PAGE + 1;
+  // the page kernel's instance for what the call wants per token (behind the normalizer: byte offsets of the normalized
+  // document, mapped back by norm_offsets_kernel)
+  const bool offs = flags & B2T_WANT_OFFSETS;
+  const unsigned lay = (offs ? L_OFFSETS : 0u) | ((flags & B2T_WANT_WORD_IDS) ? L_WORD_IDS : 0u) |
+                       (offs && ((flags & B2T_OFFSETS_BYTES) || ws.norm_active) ? L_BYTE_OFFSETS : 0u) |
+                       (offs && b.prefix_bits ? L_PREFIX : 0u) | (added && (flags & B2T_FLAG_ADDED_IDS) ? L_ADDED_IDS : 0u);
+  const int li = model_layout_index(lay);
+  if (li < 0) return fail(B2T_ERR_INVALID, "no page kernel for output layout %u", lay);
   ModelParams P;
   P.bytes = b.bytes; P.n = b.n;
   P.start_bits = ws.start_bits.as<uint32_t>(); P.drop_bits = ws.drop_bits.as<uint32_t>(); P.doc_bits = ws.doc_bits.as<uint32_t>();
   P.soft_bits = ws.soft_bits.as<uint32_t>(); P.page_soft = ws.page_soft.as<uint8_t>();
   P.page_carry = ws.page_carry.as<uint64_t>(); P.block_carry = ws.block_carry.as<uint64_t>(); P.page_first_doc = ws.page_first_doc.as<uint32_t>();
   P.doc_off = b.doc_off; P.n_docs = b.n_docs;
-  P.flags = ((flags & B2T_WANT_OFFSETS) ? F_OFFSETS : 0u) | ((flags & B2T_WANT_WORD_IDS) ? F_WORD_IDS : 0u) |
-            (((flags & B2T_OFFSETS_BYTES) || ws.norm_active) ? F_BYTE_OFFSETS : 0u);   // behind the normalizer: bytes of the normalized document, mapped back by norm_offsets_kernel
   P.ids = ws.tmp_ids.as<uint32_t>(); P.offsets = ws.tmp_offsets.as<uint32_t>(); P.word_ids = ws.tmp_word_ids.as<uint32_t>();
   P.row_ptr = ws.row_ptr_local.as<uint64_t>();
   P.tile_count = ws.tile_count.as<uint32_t>(); P.tile_first = ws.tile_first.as<uint32_t>();
@@ -845,16 +853,16 @@ static void model_and_count(b2t_engine* e, Workspace& ws, const Batch& b, uint32
   P.wcache = ws.wcache.as<uint4>(); P.wcache_mask = WCACHE_SLOTS - 1; P.wcache_on = e->wcache_on;
   P.prefix_bits = b.prefix_bits;
   P.added_bits = added ? ws.added_bits.as<uint32_t>() : nullptr; P.added_head = ws.added_head.as<uint32_t>(); P.added_pool = ws.added_pool.as<uint2>();
-  P.flag_added = (flags & B2T_FLAG_ADDED_IDS) ? 1u : 0u;
   P.t = e->dt;
-  if (e->model == B2T_MODEL_BPE) model_tile_kernel<MODEL_BPE><<<(unsigned)n_pages, MODEL_THREADS, 0, st>>>(P);
-  else model_tile_kernel<MODEL_WORDPIECE><<<(unsigned)n_pages, MODEL_THREADS, 0, st>>>(P);
+  const ModelKernel k = e->model == B2T_MODEL_BPE ? model_kernel<MODEL_BPE>(li) : model_kernel<MODEL_WORDPIECE>(li);
+  k<<<(unsigned)n_pages, MODEL_THREADS, 0, st>>>(P);
   rec(e, st, e->model == B2T_MODEL_BPE ? "bpe_tile" : "wordpiece_tile"); e->last_launches++;
   const int64_t n_tblk = (n_pages + TSCAN - 1) / TSCAN;
   tile_scan_block_kernel<<<(unsigned)n_tblk, TSCAN, 0, st>>>(ws.tile_count.as<uint32_t>(), ws.tile_lexcl.as<unsigned long long>(),
                                                            ws.tile_bsum.as<unsigned long long>(), n_pages);
   tile_scan_top_kernel<<<1, TSCAN, 0, st>>>(ws.tile_bsum.as<unsigned long long>(), n_tblk, &ctl->total);
   e->last_launches += 2;
+  return B2T_OK;
 }
 
 // The compaction into the workspace's CSR (unless the caller finishes into its own buffers), then in dense mode the longest
@@ -920,8 +928,7 @@ static int run_device_pipeline(b2t_engine* e, Workspace& ws, cudaStream_t st) {
   if ((rc = scan(e, ws, b, added, st))) return rc;
   if (model_pass) {
     if (e->model == B2T_MODEL_BPE) long_pretokens(e, ws, b, st);
-    model_and_count(e, ws, b, q.flags, added, st);
-    if ((rc = finish_tail(e, ws, st))) return rc;
+    if ((rc = model_and_count(e, ws, b, q.flags, added, st)) || (rc = finish_tail(e, ws, st))) return rc;
   }
   CU(cudaGetLastError());
   return B2T_OK;

@@ -21,6 +21,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <type_traits>
+#include <utility>
 #include "b2t_tables.h"
 #include "added_kernels.cuh"
 #include "long_kernels.cuh"
@@ -32,8 +33,21 @@ constexpr int TILE = PAGE;
 constexpr int MODEL_THREADS = 256;
 constexpr int THREAD_PATH_MAX = 32;  // pre-tokens up to this many bytes are merged by an 8-lane group, longer ones by a warp
 enum { MODEL_BPE = 0, MODEL_WORDPIECE = 1 };
-enum { F_OFFSETS = 1u, F_WORD_IDS = 2u, F_BYTE_OFFSETS = 4u };
 constexpr int MAX_LONG_PER_PAGE = TILE / (LONG_PRETOK_MIN + 1) + 1;  // 8
+
+// What a call writes per token, a template parameter of the page kernel: offsets (char offsets unless L_BYTE_OFFSETS),
+// word ids, the mapping of offsets back across an inserted prefix space (L_PREFIX), bit 31 on the ids of added tokens
+// (L_ADDED_IDS).  Each layout is an instance of its own, so code for outputs a call does not want takes no registers
+// (one instance with runtime flags ran at 32 registers with spills).  MODEL_LAYOUTS lists every mask a call can form:
+// byte offsets and the prefix mapping only come with offsets.
+enum : unsigned { L_OFFSETS = 1u, L_WORD_IDS = 2u, L_BYTE_OFFSETS = 4u, L_PREFIX = 8u, L_ADDED_IDS = 16u };
+constexpr unsigned MODEL_LAYOUTS[] = {0u, 1u, 5u, 9u, 13u, 2u, 3u, 7u, 11u, 15u, 16u, 17u, 21u, 25u, 29u, 18u, 19u, 23u, 27u, 31u};
+constexpr int N_MODEL_LAYOUTS = (int)(sizeof(MODEL_LAYOUTS) / sizeof(MODEL_LAYOUTS[0]));
+constexpr int model_layout_index(unsigned lay) {
+  for (int i = 0; i < N_MODEL_LAYOUTS; ++i)
+    if (MODEL_LAYOUTS[i] == lay) return i;
+  return -1;
+}
 
 struct ModelParams {
   const uint8_t* bytes; int64_t n;
@@ -43,7 +57,6 @@ struct ModelParams {
   const uint32_t* soft_bits; const uint8_t* page_soft;
   const uint64_t* page_carry; const uint64_t* block_carry; const uint32_t* page_first_doc;
   const uint64_t* doc_off; uint32_t n_docs;
-  uint32_t flags;
   uint32_t* ids; uint32_t* offsets; uint32_t* word_ids; uint64_t* row_ptr;
   // pass 1 writes the tokens of page t at the provisional slots [tile_first[t], tile_first[t] + tile_count[t]) of ids / offsets /
   // word_ids (first pre-token start of the page: a page never has more tokens than bytes up to the next page's first start),
@@ -57,8 +70,8 @@ struct ModelParams {
   // ByteLevel add_prefix_space: bit p set <=> byte p of the (re-packed) batch is an inserted prefix space (else NULL)
   const uint32_t* prefix_bits;
   // added-token extraction (added_kernels.cuh): bit p <=> an added token's span starts at byte p, its id is in the list of
-  // the page; NULL when the batch did not go through the extraction.  flag_added: mark those tokens with bit 31 of the id.
-  const uint32_t* added_bits; const uint32_t* added_head; const uint2* added_pool; uint32_t flag_added;
+  // the page; NULL when the batch did not go through the extraction.  (L_ADDED_IDS: mark those tokens with bit 31 of the id.)
+  const uint32_t* added_bits; const uint32_t* added_head; const uint2* added_pool;
   DeviceTables t;
 };
 
@@ -73,8 +86,10 @@ __device__ __forceinline__ uint64_t merge_lookup(const DeviceTables& t, uint32_t
   }
 }
 
-// exclusive prefix of popcounts over nw (<= 96) words, by one full warp; returns the total
-__device__ __forceinline__ int warp_prefix_words(const uint32_t* bits, uint16_t* pref, int nw, int lane) {
+// exclusive prefix of popcounts over nw (<= 96) words, by one full warp (lane writes pref[3 lane .. 3 lane + 2]); returns
+// the total
+template <class T>
+__device__ __forceinline__ int warp_prefix_words(const uint32_t* bits, T* pref, int nw, int lane) {
   int c0 = 0, c1 = 0, c2 = 0;
   int i = lane * 3;
   if (i < nw) c0 = __popc(bits[i]);
@@ -87,13 +102,14 @@ __device__ __forceinline__ int warp_prefix_words(const uint32_t* bits, uint16_t*
     if (lane >= s) inc += o;
   }
   int ex = inc - tot;
-  if (i < nw) pref[i] = (uint16_t)ex;
-  if (i + 1 < nw) pref[i + 1] = (uint16_t)(ex + c0);
-  if (i + 2 < nw) pref[i + 2] = (uint16_t)(ex + c0 + c1);
+  if (i < nw) pref[i] = (T)ex;
+  if (i + 1 < nw) pref[i + 1] = (T)(ex + c0);
+  if (i + 2 < nw) pref[i + 2] = (T)(ex + c0 + c1);
   return __shfl_sync(0xFFFFFFFFu, inc, 31);
 }
 
 __device__ __forceinline__ uint32_t mask_le(int b) { return b >= 31 ? 0xFFFFFFFFu : ((2u << b) - 1u); }
+__device__ __forceinline__ uint32_t mask_lt(int b) { return (1u << b) - 1u; }   // b in [0, 32)
 
 // One word per byte position of the page: token id (low 20 bits) and token length in bytes (high 12 bits); length 0 =
 // no token starts here.  (Ids and lengths used to be two arrays; one array leaves 4.5 KB of the SM's shared memory /
@@ -355,23 +371,28 @@ __device__ __forceinline__ bool bit_at(const uint32_t* bits, int x) { return (bi
 // Shared memory of one page, laid out without padding.  byte / tok: the page + halo and the token starting at each
 // position (tok_pack).  Bitmaps, one bit per position: startb = units of merging (splits of the pre-tokenizer + exact
 // cuts of long ones), keptb = splits the reference keeps (word ids), leadb = first bytes of characters, tokb = token
-// starts, dsb = document starts, addedb = added-token spans; apref / spref / lpref / tpref = exclusive prefix of the
-// popcounts of startb / keptb / leadb / tokb per word.  dlast: last doc start before each word of the page, or -1.
-// pt: the page's pre-token starts, then the end of the last one.  list: pre-tokens the word cache did not resolve, then
-// the positions of the tokens.  BPE: mq = pre-tokens of 33..256 bytes; lk / lcum / loff = the long pre-tokens starting
-// in the page (indices in position order, exclusive prefix of their token counts, place in long_out).
+// starts, dsb = document starts, addedb = added-token spans; apref / spref / lpref = exclusive prefix of the popcounts of
+// startb / keptb / leadb per word; tpref = the page's tokens before each word, the long pre-tokens' included (a long
+// pre-token covers the rest of its word, so its tokens come after every token of that word and before the next word's).
+// Per word of the page, the document in force at its first position: dlast = its start, or -1 when it began in an
+// earlier page; dcb / dwb = chars / kept splits of the page before that start (negative: the carry of the earlier
+// pages, carry_c / carry_w).  pt: the page's pre-token starts, then the end of the last one.  list: pre-tokens the word
+// cache did not resolve.  BPE: mq = pre-tokens of 33..256 bytes; lk / lcum / loff = the long pre-tokens starting in the
+// page (indices in position order, exclusive prefix of their token counts, place in long_out).
 template <int HALO_>
 struct PageCommon {
   static constexpr int HALO = HALO_, SPAN = TILE + HALO, NW = SPAN / 32, TW = TILE / 32;
   static_assert(NW <= 96 && SPAN % 16 == 0, "warp_prefix_words handles <= 96 words; tok is 16-byte aligned");
+  static_assert(2 * TW <= MODEL_THREADS, "stage_page: one thread per word of the page for pt, one for dcb / dwb");
   uint8_t byte[SPAN];
   uint32_t tok[SPAN];
   long long span_doc_start;  // first byte of the document that spans into this page
   uint32_t startb[NW + 1], keptb[NW + 1], leadb[NW + 1], tokb[NW + 1], dsb[TW + 1], addedb[TW + 1];
-  uint16_t apref[NW + 1], spref[NW + 1], lpref[NW + 1], tpref[NW + 1];
+  int tpref[NW + 1], dcb[TW], dwb[TW];
+  uint16_t apref[NW + 1], spref[NW + 1], lpref[NW + 1];
   int16_t dlast[TW + 1];
   uint16_t pt[TILE + 2], list[SPAN];
-  int tile, npt, elast, is_long, ntok, nmiss;
+  int tile, npt, elast, is_long, ntok, nmiss, carry_c, carry_w;
 };
 struct BpePage : PageCommon<256> {
   uint16_t mq[TILE / THREAD_PATH_MAX + 2], lk[MAX_LONG_PER_PAGE + 1];
@@ -383,15 +404,6 @@ struct WpPage : PageCommon<416> {
   int next, long_chars;
 };
 template <int MODEL> using PageState = std::conditional_t<MODEL == MODEL_BPE, BpePage, WpPage>;
-
-// Tokens of long pre-tokens (resolved by the pre-pass) that precede page position x.  A long WordPiece split is the
-// page's last token.
-__device__ __forceinline__ int long_tokens_before(const BpePage& sh, int x) {
-  int c = 0;
-  for (int a = 0; a < sh.nl; ++a) if ((int)sh.pt[sh.lk[a]] < x) c = sh.lcum[a + 1];
-  return c;
-}
-__device__ __forceinline__ int long_tokens_before(const WpPage&, int) { return 0; }
 
 // [s, e) is a piece of a cut pre-token (not a whole split of the pre-tokenizer): with ignore_merges the whole-word rule
 // and the word cache (whose entries follow that rule) do not apply to it
@@ -441,56 +453,61 @@ __device__ __forceinline__ int64_t char_boundary(const ModelParams& P, int64_t g
 
 // Where a token's document starts, seen from the page position x where the token's pre-token starts: ds = its first
 // byte, cb = chars of the page before it (negative: it started in an earlier page), wid = the pre-token's word id.
+// Shared-memory reads of the facts stage_page keeps per word; only a doc start in x's own word is ranked here.
 struct DocOrigin { int64_t ds; int cb; uint32_t wid; };
-template <class S>
-__device__ __forceinline__ DocOrigin doc_origin(const ModelParams& P, const S& sh, int64_t base, int x) {
-  const int xx = x < TILE ? x : TILE - 1;
-  const uint32_t m = sh.dsb[xx >> 5] & mask_le(xx & 31);
-  const int D = m ? (xx & ~31) + 31 - __clz((int)m) : (int)sh.dlast[xx >> 5];  // last doc start at or before x in the page, or -1
-  int2 carry = make_int2(0, 0);
-  if (D < 0) {  // chars / kept splits of the document before this page, counted from its start (pretok_kernels.cuh K1b)
-    const uint64_t c = __ldg(P.page_carry + sh.tile);
-    const uint64_t bc = (c >> 31) & 1ull ? 0ull : __ldg(P.block_carry + (sh.tile >> 10));  // + the scan block's carry
-    carry = make_int2((int)(((uint32_t)c & 0x7FFFFFFFu) + (uint32_t)bc), (int)((uint32_t)(c >> 32) + (uint32_t)(bc >> 32)));
-  }
+template <unsigned LAY, class S>
+__device__ __forceinline__ DocOrigin doc_origin(const S& sh, int64_t base, int x) {
+  const int xx = x < TILE ? x : TILE - 1, w = xx >> 5;
+  const uint32_t m = sh.dsb[w] & mask_le(xx & 31);
   DocOrigin o;
-  o.ds = D >= 0 ? base + D : sh.span_doc_start;
-  o.cb = D >= 0 ? bit_rank_incl(sh.lpref, sh.leadb, D) - 1 : -carry.x;
-  // kept splits before the doc start (the split AT the doc start may itself be removed whitespace)
-  const int wb = D >= 0 ? bit_rank_incl(sh.spref, sh.keptb, D) - (int)bit_at(sh.keptb, D) : -carry.y;
-  o.wid = (uint32_t)(bit_rank_incl(sh.spref, sh.keptb, x) - 1 - wb);
+  int wb;  // kept splits before the doc start (the split AT the doc start may itself be removed whitespace)
+  if (m) {  // the last doc start at or before x is in x's word
+    const int D = (xx & ~31) + 31 - __clz((int)m);
+    o.ds = base + D;
+    o.cb = bit_rank_incl(sh.lpref, sh.leadb, D) - 1;
+    wb = bit_rank_incl(sh.spref, sh.keptb, D) - (int)bit_at(sh.keptb, D);
+  } else {
+    const int D = sh.dlast[w];
+    o.ds = D >= 0 ? base + D : sh.span_doc_start;
+    o.cb = sh.dcb[w];
+    wb = sh.dwb[w];
+  }
+  o.wid = (LAY & L_WORD_IDS) ? (uint32_t)(bit_rank_incl(sh.spref, sh.keptb, x) - 1 - wb) : 0u;
   return o;
 }
 
 // Offsets and word id of the token in slot `out`: c0 / c1 = chars of the page before its first char / up to its end
 // (for char offsets); g0 / g1 = its bytes in the batch (for byte offsets, widened to whole characters).
+template <unsigned LAY>
 __device__ __forceinline__ void place_token(const ModelParams& P, const DocOrigin& o, unsigned long long out,
                                             int c0, int c1, int64_t g0, int64_t g1) {
-  if (P.flags & F_OFFSETS) {
-    const bool byte_off = P.flags & F_BYTE_OFFSETS;
+  if constexpr ((LAY & L_OFFSETS) != 0) {
+    constexpr bool byte_off = (LAY & L_BYTE_OFFSETS) != 0;
     uint32_t o0, o1;
-    if (!byte_off) {
+    if constexpr (!byte_off) {
       o0 = (uint32_t)(c0 - o.cb); o1 = (uint32_t)(c1 - o.cb);
     } else {
       o0 = (uint32_t)(char_boundary(P, g0, -1) - o.ds); o1 = (uint32_t)(char_boundary(P, g1, 1) - o.ds);
     }
-    if (P.prefix_bits && ((__ldg(P.prefix_bits + (o.ds >> 5)) >> (o.ds & 31)) & 1u)) {
-      // offsets were computed on the document WITH its inserted space: map back (normalizer.rs:503-514)
-      if (o1 == 1u && byte_off) o1 = (uint32_t)(char_boundary(P, o.ds + 2, 1) - o.ds);  // the space alone: its whole first character
-      o0 = o0 ? o0 - 1u : 0u;
-      o1 = o1 > 2u ? o1 - 1u : 1u;
+    if constexpr ((LAY & L_PREFIX) != 0) {
+      if ((__ldg(P.prefix_bits + (o.ds >> 5)) >> (o.ds & 31)) & 1u) {
+        // offsets were computed on the document WITH its inserted space: map back (normalizer.rs:503-514)
+        if (o1 == 1u && byte_off) o1 = (uint32_t)(char_boundary(P, o.ds + 2, 1) - o.ds);  // the space alone: its whole first character
+        o0 = o0 ? o0 - 1u : 0u;
+        o1 = o1 > 2u ? o1 - 1u : 1u;
+      }
     }
     reinterpret_cast<uint2*>(P.offsets)[out] = make_uint2(o0, o1);
   }
-  if (P.flags & F_WORD_IDS) P.word_ids[out] = o.wid;
+  if constexpr ((LAY & L_WORD_IDS) != 0) P.word_ids[out] = o.wid;
 }
 
 // A token of the page logic (and a long WordPiece split's [UNK]) that starts at page position ts: c1 / g1 as above.
-template <class S>
+template <unsigned LAY, class S>
 __device__ __forceinline__ void emit_token(const ModelParams& P, const S& sh, int64_t base, unsigned long long out,
                                            uint32_t id, int ts, int c1, int64_t g1) {
-  P.ids[out] = (P.flag_added && ts < TILE && added_at(P, sh, ts)) ? (id | 0x80000000u) : id;
-  place_token(P, doc_origin(P, sh, base, ts), out, bit_rank_incl(sh.lpref, sh.leadb, ts) - 1, c1, base + ts, g1);
+  P.ids[out] = ((LAY & L_ADDED_IDS) && ts < TILE && bit_at(sh.addedb, ts)) ? (id | 0x80000000u) : id;
+  place_token<LAY>(P, doc_origin<LAY>(sh, base, ts), out, bit_rank_incl(sh.lpref, sh.leadb, ts) - 1, c1, base + ts, g1);
 }
 
 // ------------------------------------------------------------------------------------------------ page phases
@@ -622,12 +639,22 @@ __device__ __forceinline__ void stage_page(const ModelParams& P, S& sh, int64_t 
   } else if (warp == 5 && lane == 0) {
     uint32_t fd = __ldg(P.page_first_doc + t);
     sh.span_doc_start = fd > 0 ? (long long)__ldg(P.doc_off + fd - 1) : 0;
+    // chars / kept splits of the document before this page, counted from its start (pretok_kernels.cuh K1b), + the scan
+    // block's carry
+    const uint64_t c = __ldg(P.page_carry + t);
+    const uint64_t bc = (c >> 31) & 1ull ? 0ull : __ldg(P.block_carry + (t >> 10));
+    sh.carry_c = (int)(((uint32_t)c & 0x7FFFFFFFu) + (uint32_t)bc);
+    sh.carry_w = (int)((uint32_t)(c >> 32) + (uint32_t)(bc >> 32));
   }
   __syncthreads();
-  if (tid < S::TW) {
+  if (tid < TW) {
     uint32_t bits = sh.startb[tid];
     int idx = sh.apref[tid];
     while (bits) { sh.pt[idx++] = (uint16_t)(tid * 32 + __ffs((int)bits) - 1); bits &= bits - 1u; }
+  } else if (tid < 2 * TW) {  // the document in force at the first position of word w (doc_origin)
+    const int w = tid - TW, D = sh.dlast[w];
+    sh.dcb[w] = D >= 0 ? bit_rank_incl(sh.lpref, sh.leadb, D) - 1 : -sh.carry_c;
+    sh.dwb[w] = D >= 0 ? bit_rank_incl(sh.spref, sh.keptb, D) - (int)bit_at(sh.keptb, D) : -sh.carry_w;
   }
   if (tid == 0) sh.pt[sh.npt] = (uint16_t)sh.elast;
 }
@@ -788,8 +815,8 @@ __device__ __forceinline__ void resolve_wordpiece(const ModelParams& P, WpPage& 
   }
 }
 
-// P5/P6: token bitmap, its prefix, the list of token positions and the page's token count (no ordering between pages:
-// an in-order look-back chain stalls every page behind the slowest of the pages in flight)
+// P5/P6: token bitmap, its prefix (long pre-tokens included) and the page's token count (no ordering between pages: an
+// in-order look-back chain stalls every page behind the slowest of the pages in flight)
 template <int MODEL, class S>
 __device__ __forceinline__ void count_tokens(const ModelParams& P, S& sh, int64_t t, int64_t base) {
   const int tid = threadIdx.x, lane = tid & 31;
@@ -801,32 +828,45 @@ __device__ __forceinline__ void count_tokens(const ModelParams& P, S& sh, int64_
   }
   __syncthreads();
   if (tid < 32) {
-    const int tot = warp_prefix_words(sh.tokb, sh.tpref, S::NW, lane);
-    if (lane == 0) sh.ntok = tot;
-  }
-  __syncthreads();
-  for (int row = tid >> 5; row < S::NW; row += MODEL_THREADS / 32) {
-    const uint32_t tb = sh.tokb[row];
-    if ((tb >> lane) & 1u) sh.list[sh.tpref[row] + __popc(tb & ((1u << lane) - 1u))] = (uint16_t)(row * 32 + lane);
-  }
-  if (tid == 0) {
-    P.tile_count[t] = (uint32_t)(sh.ntok + long_tokens_before(sh, TILE) + (sp.long_kept ? 1 : 0));
-    P.tile_first[t] = (uint32_t)(base + sp.first);
+    int tot = warp_prefix_words(sh.tokb, sh.tpref, S::NW, lane);
+    if constexpr (MODEL == MODEL_BPE) {
+      const int nl = sh.nl;
+      if (nl) {  // (rare) word w also follows the tokens of the long pre-tokens that start in words before it
+        for (int w = lane * 3; w < lane * 3 + 3 && w < S::NW; ++w) {
+          int c = 0;
+          for (int a = 0; a < nl; ++a) if (((int)sh.pt[sh.lk[a]] >> 5) < w) c = sh.lcum[a + 1];
+          sh.tpref[w] += c;
+        }
+        tot += sh.lcum[nl];
+      }
+    }
+    if (lane == 0) {
+      sh.ntok = tot;
+      P.tile_count[t] = (uint32_t)(tot + (sp.long_kept ? 1 : 0));
+      P.tile_first[t] = (uint32_t)(base + sp.first);
+    }
   }
 }
 
-// P7: ids, offsets and word ids of the page's tokens at the provisional slots from base + first on
-template <int MODEL, class S>
+// the page's tokens (long pre-tokens' included) before page position x < SPAN
+template <class S>
+__device__ __forceinline__ int tokens_before(const S& sh, int x) { return sh.tpref[x >> 5] + __popc(sh.tokb[x >> 5] & mask_lt(x & 31)); }
+
+// P7: ids, offsets and word ids of the page's tokens at the provisional slots from base + first on.  A warp takes a word
+// of tokb, a lane the token that starts at its position: its slot is the word's prefix plus its rank in the word.
+template <int MODEL, unsigned LAY, class S>
 __device__ __forceinline__ void emit_tokens(const ModelParams& P, const S& sh, int64_t base) {
   const PageSpan sp = page_span<MODEL>(sh);
   const unsigned long long excl = (unsigned long long)(base + sp.first);
-  const int n_normal = sh.ntok;
-  for (int j = threadIdx.x; j < n_normal; j += MODEL_THREADS) {
-    const int pos = sh.list[j];
+  const int lane = threadIdx.x & 31;
+  for (int row = threadIdx.x >> 5; row < S::NW; row += MODEL_THREADS / 32) {
+    const uint32_t tb = sh.tokb[row];
+    if (!((tb >> lane) & 1u)) continue;
+    const int pos = row * 32 + lane;
     const uint32_t tk = sh.tok[pos];
     const int e = pos + tok_len(tk);
-    emit_token(P, sh, base, excl + (unsigned long long)(j + long_tokens_before(sh, pos)), tok_id(tk), pos,
-               bit_rank_incl(sh.lpref, sh.leadb, e - 1), base + e);
+    emit_token<LAY>(P, sh, base, excl + (unsigned long long)(sh.tpref[row] + __popc(tb & mask_lt(lane))), tok_id(tk), pos,
+                    bit_rank_incl(sh.lpref, sh.leadb, e - 1), base + e);
   }
   if constexpr (MODEL == MODEL_BPE) {
     // tokens of the long pre-tokens, produced by the pre-pass (positions relative to the pre-token start)
@@ -835,21 +875,20 @@ __device__ __forceinline__ void emit_tokens(const ModelParams& P, const S& sh, i
       const int ntl = sh.lcum[a + 1] - sh.lcum[a];
       if (ntl == 0) continue;
       const uint4* __restrict__ lo = P.long_out + sh.loff[a];
-      const int nb = ls == 0 ? 0 : bit_rank_incl(sh.tpref, sh.tokb, ls - 1);
-      const unsigned long long obase = excl + (unsigned long long)(nb + sh.lcum[a]);
+      const unsigned long long obase = excl + (unsigned long long)tokens_before(sh, ls);
       const int X = bit_rank_incl(sh.lpref, sh.leadb, ls) - 1;  // chars of the page before the pre-token
-      const DocOrigin o = doc_origin(P, sh, base, ls);
+      const DocOrigin o = doc_origin<LAY>(sh, base, ls);
       for (int k = threadIdx.x; k < ntl; k += MODEL_THREADS) {
         const uint4 r = lo[k];
         P.ids[obase + k] = r.x;
-        place_token(P, o, obase + k, X + (int)r.z, X + (int)r.w, base + ls + (k ? (int64_t)lo[k - 1].y : 0), base + ls + (int64_t)r.y);
+        place_token<LAY>(P, o, obase + k, X + (int)r.z, X + (int)r.w, base + ls + (k ? (int64_t)lo[k - 1].y : 0), base + ls + (int64_t)r.y);
       }
     }
   } else if (sp.long_kept && threadIdx.x == 0) {
     // chars up to the end of the long split = chars before it in the page + its own
     const int ls = sh.pt[sh.npt - 1];
-    emit_token(P, sh, base, excl + (unsigned long long)sh.ntok, P.t.unk_id, ls,
-               bit_rank_incl(sh.lpref, sh.leadb, ls) - 1 + sh.long_chars, sh.long_end);
+    emit_token<LAY>(P, sh, base, excl + (unsigned long long)sh.ntok, P.t.unk_id, ls,
+                    bit_rank_incl(sh.lpref, sh.leadb, ls) - 1 + sh.long_chars, sh.long_end);
   }
 }
 
@@ -861,13 +900,12 @@ __device__ __forceinline__ void write_row_ptr(const ModelParams& P, const S& sh,
     const int64_t pos = (int64_t)__ldg(P.doc_off + d) - base;
     if (pos >= TILE) break;
     // tokens that start before `pos` (a doc start is a pre-token start, so no token straddles it)
-    const int before = pos == 0 ? 0 : bit_rank_incl(sh.tpref, sh.tokb, (int)pos - 1);
-    P.row_ptr[d] = (unsigned long long)(before + long_tokens_before(sh, (int)pos));
+    P.row_ptr[d] = (unsigned long long)tokens_before(sh, (int)pos);
   }
 }
 
 constexpr int MODEL_MINBLOCKS = 8;  // 8 blocks/SM (32 regs, small spills) rather than 5 (48 regs): the kernel is latency-bound
-template <int MODEL>
+template <int MODEL, unsigned LAY>
 __global__ void __launch_bounds__(MODEL_THREADS, MODEL_MINBLOCKS) model_tile_kernel(const ModelParams P) {
   __shared__ __align__(16) PageState<MODEL> sh;
   const int tid = threadIdx.x;
@@ -893,8 +931,20 @@ __global__ void __launch_bounds__(MODEL_THREADS, MODEL_MINBLOCKS) model_tile_ker
   __syncthreads();
   count_tokens<MODEL>(P, sh, t, base);
   __syncthreads();
-  emit_tokens<MODEL>(P, sh, base);
+  emit_tokens<MODEL, LAY>(P, sh, base);
   write_row_ptr(P, sh, t, base);
+}
+
+// The instances of one model, in the order of MODEL_LAYOUTS
+using ModelKernel = void (*)(const ModelParams);
+template <int MODEL, int... I>
+struct ModelKernelTable { static constexpr ModelKernel k[sizeof...(I)] = {&model_tile_kernel<MODEL, MODEL_LAYOUTS[I]>...}; };
+template <int MODEL, int... I>
+constexpr ModelKernelTable<MODEL, I...> model_kernel_table(std::integer_sequence<int, I...>) { return {}; }
+template <int MODEL>
+__host__ inline ModelKernel model_kernel(int layout_index) {
+  using T = decltype(model_kernel_table<MODEL>(std::make_integer_sequence<int, N_MODEL_LAYOUTS>{}));
+  return T::k[layout_index];
 }
 
 
