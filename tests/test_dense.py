@@ -1,42 +1,14 @@
 """Dense mode (b2t_encode_batch_dense*): special-token template + truncation + padding on the device.
 CPU: the oracle-side restatement (oracle.dense_rows) against the reference wheel.  GPU: the engine against both."""
-import ctypes, json, os
+import ctypes, json
 import numpy as np
 import pytest
-import helpers, fuzzgen, corpus
+import corpus
+import dense_cases as dc
+from dense_cases import tk
 from oracle import oracle as orc
 
-tk = helpers.wheel()
-
-TEMPLATES = {
-    "gpt2_style": lambda v: {"type": "TemplateProcessing",
-                             "single": [{"SpecialToken": {"id": "<s>", "type_id": 0}}, {"Sequence": {"id": "A", "type_id": 0}},
-                                        {"SpecialToken": {"id": "</s>", "type_id": 0}}, {"SpecialToken": {"id": "<s>", "type_id": 0}}],
-                             "pair": [{"Sequence": {"id": "A", "type_id": 0}}, {"Sequence": {"id": "B", "type_id": 1}}],
-                             "special_tokens": {"<s>": {"id": "<s>", "ids": [v["a"]], "tokens": ["a"]},
-                                                "</s>": {"id": "</s>", "ids": [v["b"], v["c"]], "tokens": ["b", "c"]}}},
-    "wordpiece": lambda v: {"type": "BertProcessing", "sep": ["[SEP]", v["[SEP]"]], "cls": ["[CLS]", v["[CLS]"]]},
-    "llama3_style": lambda v: None,
-}
-# (truncation | None, padding)
-SETTINGS = [
-    (dict(max_length=16, direction="right"), dict(length=16, direction="right", pad_id=0)),
-    (dict(max_length=12, direction="left"), dict(length=None, direction="left", pad_id=3)),
-    (dict(max_length=40, direction="right"), dict(length=None, direction="right", pad_id=1, pad_to_multiple_of=8)),
-    (None, dict(length=None, direction="right", pad_id=2)),
-    (dict(max_length=7, direction="right"), dict(length=20, direction="left", pad_id=5, pad_to_multiple_of=16)),
-]
-
-
-def tokenizer_json(name):
-    js = json.loads(helpers.asset_json(name))
-    pp = TEMPLATES[name](js["model"]["vocab"])
-    js["post_processor"] = pp
-    return json.dumps(js)
-
-
-def docs_for(seed):
-    return fuzzgen.rand_docs(seed, 600, max_len=120) + ["", " ", "a", "hello world " * 30]
+SETTINGS = dc.DENSE_SETTINGS
 
 
 def spec_of(js, tr, pd):
@@ -49,40 +21,25 @@ def spec_of(js, tr, pd):
                 pad_id=pd["pad_id"], truncate_left=bool(tr and tr["direction"] == "left"), pad_left=pd["direction"] == "left", pre=pre, post=post)
 
 
-def wheel_dense(js, docs, tr, pd):
-    tok = tk.Tokenizer.from_str(js)
-    if tr:
-        tok.enable_truncation(tr["max_length"], direction=tr["direction"])
-    tok.enable_padding(direction=pd["direction"], pad_id=pd["pad_id"], length=pd["length"], pad_to_multiple_of=pd.get("pad_to_multiple_of"))
-    encs = tok.encode_batch(docs)
-    return (np.array([e.ids for e in encs], dtype=np.uint32).reshape(len(docs), -1),
-            np.array([e.attention_mask for e in encs], dtype=np.uint8).reshape(len(docs), -1))
-
-
 @pytest.mark.skipif(tk is None, reason="reference wheel not importable")
-@pytest.mark.parametrize("name", list(TEMPLATES))
+@pytest.mark.parametrize("name", dc.DENSE_NAMES)
 def test_oracle_dense_matches_wheel(name):
-    js = tokenizer_json(name)
+    js = dc.tokenizer_json(name)
     o = orc.Oracle(js)
-    docs = docs_for(11)
+    docs = dc.docs_for(11)
     ids, _, _, rp = o.encode_batch(docs)
     for tr, pd in SETTINGS:
         got = orc.dense_rows(ids, rp, **spec_of(js, tr, pd))
-        exp = wheel_dense(js, docs, tr, pd)
-        assert np.array_equal(got[0], exp[0]) and np.array_equal(got[1], exp[1]), (name, tr, pd)
-        assert np.array_equal(got[2], exp[1].sum(axis=1))
+        exp = dc.wheel_rows(js, docs, tr, pd)
+        assert np.array_equal(got[0], exp[0]) and np.array_equal(got[1], exp[2]), (name, tr, pd)
+        assert np.array_equal(got[2], exp[3])
 
 
-def _golden():
-    import gzip
-    return json.loads(gzip.open(os.path.join(helpers.GOLDEN, "golden_dense.json.gz")).read().decode("utf-8"))
-
-
-@pytest.mark.parametrize("name", list(TEMPLATES))
+@pytest.mark.parametrize("name", dc.DENSE_NAMES)
 def test_oracle_dense_matches_golden(name):
     """the same restatement against committed vectors of the wheel (no wheel needed)"""
-    g = _golden()
-    js = tokenizer_json(name)
+    g = dc.golden("dense")
+    js = dc.tokenizer_json(name)
     ids, _, _, rp = orc.Oracle(js).encode_batch(g["docs"])
     for k, (tr, pd) in enumerate(SETTINGS):
         c = g["cases"][f"{name}/{k}"]
@@ -90,38 +47,31 @@ def test_oracle_dense_matches_golden(name):
         assert list(got[0].shape) == c["shape"] and got[0].reshape(-1).tolist() == c["ids"] and got[2].tolist() == c["lengths"], (name, k)
 
 
-def _apply(tok, tr, pd):
-    tok.no_truncation(); tok.no_padding()
-    if tr:
-        tok.enable_truncation(tr["max_length"], direction=tr["direction"])
-    tok.enable_padding(direction=pd["direction"], pad_id=pd["pad_id"], length=pd["length"], pad_to_multiple_of=pd.get("pad_to_multiple_of"))
-
-
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", list(TEMPLATES))
+@pytest.mark.parametrize("name", dc.DENSE_NAMES)
 def test_gpu_dense_matches_oracle_and_wheel(name):
     from tokenizers_b200 import Tokenizer
-    js = tokenizer_json(name)
+    js = dc.tokenizer_json(name)
     tok, o = Tokenizer.from_str(js), orc.Oracle(js)
-    docs = docs_for(12)
+    docs = dc.docs_for(12)
     ids, _, _, rp = o.encode_batch(docs)
     for tr, pd in SETTINGS:
-        _apply(tok, tr, pd)
+        dc.apply(tok, tr, pd)
         got = tok.encode_batch_dense(docs)
         exp = orc.dense_rows(ids, rp, **spec_of(js, tr, pd))
         assert got["input_ids"].shape == exp[0].shape, (name, tr, pd)
         assert np.array_equal(got["input_ids"], exp[0]) and np.array_equal(got["attention_mask"], exp[1]) and np.array_equal(got["lengths"], exp[2]), (name, tr, pd)
         if tk is not None:
-            w = wheel_dense(js, docs, tr, pd)
-            assert np.array_equal(got["input_ids"], w[0]) and np.array_equal(got["attention_mask"], w[1]), (name, tr, pd, "wheel")
-    g = _golden()   # and the committed vectors of the wheel
+            w = dc.wheel_rows(js, docs, tr, pd)
+            assert np.array_equal(got["input_ids"], w[0]) and np.array_equal(got["attention_mask"], w[2]), (name, tr, pd, "wheel")
+    g = dc.golden("dense")   # and the committed vectors of the wheel
     for k, (tr, pd) in enumerate(SETTINGS):
-        _apply(tok, tr, pd)
+        dc.apply(tok, tr, pd)
         got = tok.encode_batch_dense(g["docs"])
         c = g["cases"][f"{name}/{k}"]
         assert list(got["input_ids"].shape) == c["shape"] and got["input_ids"].reshape(-1).tolist() == c["ids"] and got["lengths"].tolist() == c["lengths"], (name, k, "golden")
     # without special tokens
-    _apply(tok, *SETTINGS[0])
+    dc.apply(tok, *SETTINGS[0])
     got = tok.encode_batch_dense(docs, add_special_tokens=False, want_mask=False)
     sp = spec_of(js, *SETTINGS[0]); sp["pre"], sp["post"] = [], []
     exp = orc.dense_rows(ids, rp, **sp)
@@ -132,7 +82,7 @@ def test_gpu_dense_matches_oracle_and_wheel(name):
 def test_gpu_dense_multi_chunk_device_entry_and_errors(monkeypatch):
     from tokenizers_b200 import Tokenizer, _lib
     import torch
-    js = tokenizer_json("gpt2_style")
+    js = dc.tokenizer_json("gpt2_style")
     o = orc.Oracle(js)
     data, off = corpus.generate(2, 31, 0, 3000)
     ids, _, _, rp = o.encode_batch_csr(data, off)[0], None, None, o.encode_batch_csr(data, off)[3]
@@ -140,19 +90,19 @@ def test_gpu_dense_multi_chunk_device_entry_and_errors(monkeypatch):
     exp = orc.dense_rows(ids, rp, **spec_of(js, tr, pd))
     monkeypatch.setenv("B2T_CHUNK_BYTES", "65536")   # many chunks through the host pipeline
     tok = Tokenizer.from_str(js)
-    _apply(tok, tr, pd)
+    dc.apply(tok, tr, pd)
     got = tok.encode_batch_dense(data, off)
     assert np.array_equal(got["input_ids"], exp[0]) and np.array_equal(got["attention_mask"], exp[1])
     # BatchLongest runs as one device pass whatever the chunk size
     tr2, pd2 = dict(max_length=100, direction="left"), dict(length=None, direction="right", pad_id=9)
-    _apply(tok, tr2, pd2)
+    dc.apply(tok, tr2, pd2)
     got = tok.encode_batch_dense(data, off)
     exp2 = orc.dense_rows(ids, rp, **spec_of(js, tr2, pd2))
     assert np.array_equal(got["input_ids"], exp2[0]) and np.array_equal(got["attention_mask"], exp2[1])
     # device entry point
     L = _lib.lib()
     for trd, pdd, e in ((tr, pd, exp), (tr2, pd2, exp2)):
-        _apply(tok, trd, pdd)
+        dc.apply(tok, trd, pdd)
         sp, keep = tok.dense_spec()
         d_bytes = torch.from_numpy(np.concatenate([data, np.zeros(64, np.uint8)])).cuda()
         d_off = torch.from_numpy(off.astype(np.int64)).cuda()
@@ -166,10 +116,10 @@ def test_gpu_dense_multi_chunk_device_entry_and_errors(monkeypatch):
         L.b2t_result_free(res)
         assert np.array_equal(out.cpu().numpy().view(np.uint32).reshape(n, W), e[0])
     # a row that does not fit a fixed length is an error, not a silently cut row
-    _apply(tok, None, dict(length=8, direction="right", pad_id=0))
+    dc.apply(tok, None, dict(length=8, direction="right", pad_id=0))
     with pytest.raises(_lib.B2TError):
         tok.encode_batch_dense(data, off)
     # empty batch
-    _apply(tok, tr, pd)
+    dc.apply(tok, tr, pd)
     got = tok.encode_batch_dense([])
     assert got["input_ids"].shape == (0, 64)
