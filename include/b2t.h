@@ -267,6 +267,65 @@ const uint8_t* b2t_result_type_ids(const b2t_result* r);
 int b2t_pre_tokenize_batch(b2t_engine* e, const uint8_t* bytes, const uint64_t* doc_off, uint32_t n_docs,
                            b2t_result** out);
 
+/* Decoding (tokenizer/mod.rs:935-953 decode, :1404-1416 decode_batch): ids -> text on the device, for the decoders of the
+ * pipelines the engine encodes.  Each id becomes the added vocabulary's string for it, else the model's; ids that are in
+ * neither (ids at or above the largest id, 0xFFFFFFFF, ids with bit 31) are dropped; with B2T_DECODE_SKIP_SPECIAL a token
+ * whose string is the content of a special added token is dropped.  The decoder then joins the kept tokens:
+ *   B2T_DECODER_NONE      tokens.join(" ")
+ *   B2T_DECODER_WORDPIECE decoders/wordpiece.rs:31-61: every kept token but the first loses `prefix` (or gains " "), then
+ *                         the cleanup replacements run on that token alone
+ *   B2T_DECODER_BYTELEVEL pre_tokenizers/byte_level.rs:156-171: chars -> bytes through the inverse byte map (a token with a
+ *                         char outside it contributes its UTF-8), then String::from_utf8_lossy once per row */
+typedef enum { B2T_DECODER_NONE = 0, B2T_DECODER_BYTELEVEL = 1, B2T_DECODER_WORDPIECE = 2 } b2t_decoder_kind;
+enum { B2T_ADDED_SPECIAL = 16u };       /* b2t_decoder_spec.added_flags: AddedToken.special (with the B2T_ADDED_* bits) */
+enum { B2T_DECODE_SKIP_SPECIAL = 1u };  /* decode flags: skip_special_tokens */
+typedef struct {
+  uint32_t struct_size;     /* sizeof(b2t_decoder_spec) */
+  int32_t kind;             /* b2t_decoder_kind; any other value fails with B2T_ERR_UNSUPPORTED */
+  const char* prefix;       /* WordPiece: NUL-terminated prefix ("##"); NULL = "" */
+  int32_t cleanup;          /* WordPiece: cleanup */
+  /* the whole added vocabulary (also on engines whose encode path does not extract it): token i = added_bytes[added_off[i]
+   * .. added_off[i+1]) with id added_ids[i] (< 2^20) and flags added_flags[i] (B2T_ADDED_NORMALIZED, B2T_ADDED_SPECIAL) */
+  uint32_t n_added;
+  const uint8_t* added_bytes;
+  const uint32_t* added_off;
+  const uint32_t* added_ids;
+  const uint8_t* added_flags;
+} b2t_decoder_spec;
+
+/* Sets the decoder of the engine's decode entry points (spec = NULL: none; the decode calls then fail with
+ * B2T_ERR_INVALID).  Builds one table entry per id in [0, largest id] (ids < 2^20): whether the id exists, whether
+ * skip_special_tokens drops it, and its image as the first kept token and as a later one.  Refused with
+ * B2T_ERR_UNSUPPORTED (the engine keeps no decoder; encoding is unaffected): an unknown kind, added tokens with
+ * normalized=true on an engine with a normalizer (the reference's tree and its release disagree on their string), an
+ * image over 16383 bytes.  Not to be called concurrently with decodes. */
+int b2t_engine_set_decoder(b2t_engine* e, const b2t_decoder_spec* spec);
+
+/* The table b2t_engine_set_decoder builds and the kernels read, from the configuration's vocabulary and the spec alone
+ * (host only, no device needed).  Entry id = table[id]: bits 0-31 the image's offset in pool, bits 32-45 the first
+ * image's length, bits 46-59 the later image's length (its bytes follow the first image's), bit 60 the id exists, bit 61
+ * skip_special_tokens drops it.  Call with table = pool = NULL for *n_ids and *pool_bytes, then with buffers that large. */
+int b2t_decoder_images(const b2t_config* cfg, const b2t_decoder_spec* spec, uint64_t* table, uint8_t* pool, uint32_t* n_ids,
+                       uint64_t* pool_bytes);
+
+/* Decodes n_rows rows of ids: row r = ids[row_ptr[r] .. row_len ? row_ptr[r] + row_len[r] : row_ptr[r+1]) -- the token CSR
+ * of b2t_encode_batch (row_len = NULL), or padded [n, L] rows with their lengths (row_ptr[r] = r L).  row_ptr must be
+ * non-decreasing and every row inside [0, n_ids) (B2T_ERR_INVALID otherwise).  Result: the UTF-8 text of every row back to
+ * back, row r = text[text_off[r] .. text_off[r+1]) (b2t_result_text / b2t_result_text_off; b2t_result_n_docs = n_rows,
+ * b2t_result_n_tokens = text_off[n_rows]), exactly decode(row, skip_special_tokens).  Per-call limits (B2T_ERR_TOO_LARGE):
+ * n_ids < 2^31, the images of one row (its text before the lossy step) below 2^30 bytes.  HOST buffers in, pinned host text out; the call runs in chunks of
+ * whole rows on a slot set of its own, as b2t_encode_batch does (a row larger than a chunk is a chunk of its own), and
+ * concurrently with other host calls.  Within the call only a chunk's copy of its text back overlaps the next chunk: each
+ * chunk waits for the host to read its text size (and for ByteLevel whether the lossy rewrite runs) before its text is
+ * written. */
+int b2t_decode_batch(b2t_engine* e, const uint32_t* ids, uint64_t n_ids, const uint64_t* row_ptr, const uint32_t* row_len, uint32_t n_rows,
+                     uint32_t flags, b2t_result** out);
+/* Device buffers in, device text out (owned by the engine, valid until the next device-resident call), on `stream`. */
+int b2t_decode_batch_device(b2t_engine* e, const uint32_t* d_ids, uint64_t n_ids, const uint64_t* d_row_ptr, const uint32_t* d_row_len,
+                            uint32_t n_rows, uint32_t flags, void* stream, b2t_result** out);
+const uint8_t* b2t_result_text(const b2t_result* r);       /* text_off[n_rows] bytes, NULL for results that are not decodes */
+const uint64_t* b2t_result_text_off(const b2t_result* r);  /* n_rows + 1, NULL for results that are not decodes */
+
 /* Result accessors (Encoding fields of tokenizer/encoding.rs:11-31 as one CSR over the batch).  Pointers are host
  * pointers for b2t_encode_batch / b2t_pre_tokenize_batch and device pointers for b2t_encode_batch_device. */
 uint64_t b2t_result_n_tokens(const b2t_result* r);

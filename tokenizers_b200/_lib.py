@@ -14,6 +14,9 @@ TRUNC_LONGEST_FIRST, TRUNC_ONLY_FIRST, TRUNC_ONLY_SECOND = 0, 1, 2
 PIECE_A, PIECE_B = 0x80000000, 0x80000001
 DENSE_OVERFLOW, DENSE_OFFSETS = 1, 2
 DENSE_TRIM_OFFSETS, DENSE_TRIM_PREFIX_SPACE, DENSE_SPECIAL_MASK, DENSE_SEQUENCE_IDS, DENSE_WORD_IDS = 4, 8, 16, 32, 64
+DECODER_NONE, DECODER_BYTELEVEL, DECODER_WORDPIECE = 0, 1, 2
+ADDED_SPECIAL = 16
+DECODE_SKIP_SPECIAL = 1
 
 # every symbol include/b2t.h declares
 SYMBOLS = ["b2t_engine_create", "b2t_engine_destroy", "b2t_engine_set_added_tokens", "b2t_encode_batch", "b2t_encode_batch_device", "b2t_encode_batch_device_begin",
@@ -25,7 +28,8 @@ SYMBOLS = ["b2t_engine_create", "b2t_engine_destroy", "b2t_engine_set_added_toke
            "b2t_result_special_tokens_mask", "b2t_result_sequence_ids", "b2t_result_dense_word_ids",
            "b2t_result_n_tokens", "b2t_result_n_docs", "b2t_result_on_device", "b2t_result_ids", "b2t_result_offsets",
            "b2t_result_word_ids", "b2t_result_row_ptr", "b2t_result_free", "b2t_host_alloc", "b2t_host_free",
-           "b2t_engine_set_profiling", "b2t_engine_last_kernels", "b2t_unicode_class_table", "b2t_bert_normalizer_images", "b2t_last_error", "b2t_version"]
+           "b2t_engine_set_profiling", "b2t_engine_last_kernels", "b2t_unicode_class_table", "b2t_bert_normalizer_images", "b2t_last_error", "b2t_version",
+           "b2t_engine_set_decoder", "b2t_decoder_images", "b2t_decode_batch", "b2t_decode_batch_device", "b2t_result_text", "b2t_result_text_off"]
 
 
 class Config(ctypes.Structure):
@@ -52,6 +56,11 @@ class PairDenseSpec(ctypes.Structure):
                 ("n_pieces", ctypes.c_uint32), ("piece_ids", ctypes.c_void_p), ("piece_types", ctypes.c_void_p),
                 ("want_mask", ctypes.c_uint32), ("stride", ctypes.c_uint32), ("dense_flags", ctypes.c_uint32),
                 ("overflow_type_a", ctypes.c_uint32), ("overflow_type_b", ctypes.c_uint32)]
+
+class DecoderSpec(ctypes.Structure):
+    _fields_ = [("struct_size", ctypes.c_uint32), ("kind", ctypes.c_int32), ("prefix", ctypes.c_char_p), ("cleanup", ctypes.c_int32),
+                ("n_added", ctypes.c_uint32), ("added_bytes", ctypes.c_void_p), ("added_off", ctypes.c_void_p), ("added_ids", ctypes.c_void_p),
+                ("added_flags", ctypes.c_void_p)]
 
 # the specs' size before stride and dense_flags were appended (accepted by the engine: those fields read as 0)
 DENSE_SPEC_V1_SIZE = PAIR_DENSE_SPEC_V1_SIZE = 64
@@ -105,6 +114,12 @@ def lib():
     L.b2t_engine_last_kernels.argtypes = [vp, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_float), i32]
     L.b2t_unicode_class_table.argtypes = [i32, vp]
     L.b2t_bert_normalizer_images.argtypes = [i32, vp, ctypes.c_size_t, vp]
+    L.b2t_engine_set_decoder.argtypes = [vp, ctypes.POINTER(DecoderSpec)]
+    L.b2t_decoder_images.argtypes = [ctypes.POINTER(Config), ctypes.POINTER(DecoderSpec), vp, vp, ctypes.POINTER(u32), ctypes.POINTER(u64)]
+    L.b2t_decode_batch.argtypes = [vp, vp, u64, vp, vp, u32, u32, ctypes.POINTER(vp)]
+    L.b2t_decode_batch_device.argtypes = [vp, vp, u64, vp, vp, u32, u32, vp, ctypes.POINTER(vp)]
+    for f in ("b2t_result_text", "b2t_result_text_off"):
+        getattr(L, f).argtypes = [vp]; getattr(L, f).restype = vp
     L.b2t_last_error.restype = ctypes.c_char_p
     L.b2t_version.restype = ctypes.c_char_p
     _lib = L

@@ -41,6 +41,14 @@ B2T_HDI uint32_t edge_hash(uint32_t node, uint32_t byte) {
   return h;
 }
 
+// Decoder table (decode_kernels.cuh DecodeTable, include/b2t.h b2t_decoder_images): one entry per id, x = offset of the id's
+// images in the pool, y = first image's length | later image's length << 14 | DEC_EXISTS | DEC_SKIP; the later image's
+// bytes follow the first image's
+constexpr uint32_t DEC_LEN_BITS = 14, DEC_LEN_MASK = (1u << DEC_LEN_BITS) - 1u;
+constexpr uint32_t DEC_EXISTS = 1u << 28;   // the id has a string (added vocabulary or model)
+constexpr uint32_t DEC_SKIP = 1u << 29;     // its string is the content of a special added token: skip_special_tokens drops it
+constexpr uint32_t DEC_MAX_IDS = 1u << 20;
+
 // BertNormalizer table entries (norm_kernels.cuh NormTables.ent): kind in bits 0-1
 enum { NORM_IDENT = 0u, NORM_REMOVE = 1u, NORM_STRING = 2u, NORM_SURVIVOR = 3u, NORM_MARK_FLAG = 4u, NORM_TAIL_FLAG = 0x80u };
 constexpr uint32_t NORM_LEN_MASK = 31u;   // NORM_STRING: image bytes in bits 2-6 (at most 12), pool offset in bits 8-31

@@ -22,6 +22,7 @@
 
 #include "../../include/b2t.h"
 #include "added_kernels.cuh"
+#include "decode_kernels.cuh"
 #include "dense_kernels.cuh"
 #include "host_tables.h"
 #include "long_kernels.cuh"
@@ -197,6 +198,8 @@ struct Workspace {
   DevBuf cand0, cand1, cand_any, hard_bits, inner_bits, added_bits, added_head, added_pool;
   uint32_t added_cap = 0;  // added-token extraction (added_kernels.cuh)
   DevBuf pfx_bytes, pfx_doc_off, pfx_local, pfx_block, prefix_bits, pfx_total;  // add_prefix_space re-pack (prefix_kernels.cuh)
+  // decoding (decode_kernels.cuh): staged rows (host path), D1's counts and scan, D2's text, D3's lossy counts, scan and text
+  DevBuf dec_ids, dec_row_ptr, dec_row_len, dec_count, dec_lexcl, dec_bsum, dec_text, dec_off, dec_lcount, dec_lexcl2, dec_bsum2, dec_text2, dec_off2;
   cudaStream_t stream = nullptr;
   cudaEvent_t done = nullptr;
   PinBuf h_ctl;                        // total tokens + error flag read back
@@ -217,9 +220,12 @@ struct b2t_result {
     // pairs for a pair result; n_rows = n_docs without overflowing parts)
     uint32_t dense_len = 0, n_rows = 0;
     const void* dense[N_DENSE_OUT] = {};
+    // decoding (b2t_decode_batch*): text of n_docs rows
+    const uint8_t* text = nullptr; const uint64_t* text_off = nullptr;
   } view;
   PinBuf h_ids, h_offsets, h_word_ids, h_row_ptr;  // host results own pinned memory (returned to the engine pool on free)
   PinBuf h_dense[N_DENSE_OUT];
+  PinBuf h_text, h_text_off;
 };
 
 // Publishes the dense views of a finished result: output k at buf[k] (the workspace's or the pinned result's buffers)
@@ -253,6 +259,12 @@ struct b2t_engine {
   DevBuf d_trim_vocab, d_trim_added;
   uint32_t n_trim_added = 0;
   int trim_ready = 0, added_both = 0;   // added_both: an added token has lstrip and rstrip (the rows may refuse it)
+  // decoding: the model's vocabulary as the engine received it (the decoder table is built from it and the decoder spec)
+  std::vector<uint8_t> vocab_bytes;
+  std::vector<uint32_t> vocab_off, vocab_ids;
+  int dec_on = 0, dec_kind = 0;   // b2t_engine_set_decoder
+  DecodeTable dec{};
+  DevBuf d_dec_ent, d_dec_pool;
   // Concurrency: the tables are immutable, every host-path call (b2t_encode_batch, _dense, b2t_pre_tokenize_batch) runs on a
   // slot set of its own -- NSLOT workspaces with their streams -- so calls from several host threads overlap their copies
   // and kernels; `mu` only guards the pools (and the whole call while per-kernel profiling is on: the event records are one
@@ -374,6 +386,9 @@ extern "C" int b2t_engine_create(const b2t_config* cfg, b2t_engine** out) {
     if ((rc = upload(e->d_trim_vocab, vocab_trim_counts(cfg->n_vocab, cfg->vocab_bytes, cfg->vocab_off, cfg->vocab_ids)))) return rc;
     e->trim_ready = 1;
   }
+  e->vocab_bytes.assign(cfg->vocab_bytes, cfg->vocab_bytes + cfg->vocab_off[cfg->n_vocab]);
+  e->vocab_off.assign(cfg->vocab_off, cfg->vocab_off + cfg->n_vocab + 1);
+  e->vocab_ids.assign(cfg->vocab_ids, cfg->vocab_ids + cfg->n_vocab);
   cudaError_t se = cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking);
   if (se != cudaSuccess) return fail(B2T_ERR_CUDA, "cudaStreamCreate failed: %s", cudaGetErrorString(se));
   *out = e.release();
@@ -1557,6 +1572,216 @@ extern "C" int b2t_pre_tokenize_batch(b2t_engine* e, const uint8_t* bytes, const
                    [&](b2t_engine::SlotSet& ss, uint32_t) { return pre_tokenize(e, ss, bytes, doc_off, n_docs, out); });
 }
 
+// ------------------------------------------------------------------------------------------------ decoding
+// The decoder spec, checked, -> the decoder table of a vocabulary (host only)
+static int decoder_table(const b2t_decoder_spec* sp, bool normalizer, uint32_t n_vocab, const uint8_t* vb, const uint32_t* vo, const uint32_t* vi,
+                         DecoderHost* dh) {
+  if (sp->struct_size != sizeof(b2t_decoder_spec)) return fail(B2T_ERR_INVALID, "b2t_decoder_spec: struct_size mismatch (%u != %zu)", sp->struct_size, sizeof(b2t_decoder_spec));
+  if (sp->n_added && (!sp->added_bytes || !sp->added_off || !sp->added_ids || !sp->added_flags)) return fail(B2T_ERR_INVALID, "decoder spec: null added-token list");
+  const std::string msg = build_decoder_table(sp->kind, sp->prefix, sp->cleanup != 0, normalizer, n_vocab, vb, vo, vi, sp->n_added, sp->added_bytes,
+                                              sp->added_off, sp->added_ids, sp->added_flags, dh);
+  return msg.empty() ? B2T_OK : fail(B2T_ERR_UNSUPPORTED, "%s", msg.c_str());
+}
+
+extern "C" int b2t_decoder_images(const b2t_config* cfg, const b2t_decoder_spec* spec, uint64_t* table, uint8_t* pool, uint32_t* n_ids, uint64_t* pool_bytes) {
+  if (!cfg || !spec || !n_ids || !pool_bytes || !cfg->vocab_bytes || !cfg->vocab_off || !cfg->vocab_ids) return fail(B2T_ERR_INVALID, "b2t_decoder_images: null argument");
+  DecoderHost dh;
+  int rc = decoder_table(spec, (cfg->bert_normalizer & B2T_NORM_BERT) != 0, cfg->n_vocab, cfg->vocab_bytes, cfg->vocab_off, cfg->vocab_ids, &dh);
+  if (rc) return rc;
+  *n_ids = (uint32_t)dh.ent.size(); *pool_bytes = dh.pool.size();
+  if (table) memcpy(table, dh.ent.data(), dh.ent.size() * 8);
+  if (pool) memcpy(pool, dh.pool.data(), dh.pool.size());
+  return B2T_OK;
+}
+
+extern "C" int b2t_engine_set_decoder(b2t_engine* e, const b2t_decoder_spec* spec) {
+  if (!e) return fail(B2T_ERR_INVALID, "null engine");
+  std::lock_guard<std::mutex> lk(e->dev_mu);
+  e->dec_on = 0;
+  if (!spec) return B2T_OK;
+  DecoderHost dh;
+  int rc = decoder_table(spec, e->norm_on != 0, (uint32_t)e->vocab_ids.size(), e->vocab_bytes.data(), e->vocab_off.data(), e->vocab_ids.data(), &dh);
+  if (rc) return rc;
+  CU(cudaSetDevice(e->device));
+  if ((rc = upload(e->d_dec_ent, dh.ent)) || (rc = upload(e->d_dec_pool, dh.pool))) return rc;
+  e->dec = DecodeTable{e->d_dec_ent.as<uint2>(), e->d_dec_pool.as<uint8_t>(), (uint32_t)dh.ent.size()};
+  e->dec_kind = spec->kind;
+  e->dec_on = 1;
+  return B2T_OK;
+}
+
+// D1-D3 on rows resident on the device (R), on st: *text / *text_off point at the workspace's finished text of *n_text
+// bytes.  Synchronises for the size of the text and, for ByteLevel, for whether the lossy rewrite has to run and then
+// for the rewritten size.  The profiling records name the host's reads (*_read) apart from the kernels.
+static int run_decode(b2t_engine* e, Workspace& ws, const DecodeRows& R, uint32_t flags, cudaStream_t st, const uint8_t** text, const uint64_t** text_off,
+                      uint64_t* n_text) {
+  const uint32_t n = R.n_rows, skip = (flags & B2T_DECODE_SKIP_SPECIAL) ? 1u : 0u;
+  const bool lossy = e->dec_kind == B2T_DECODER_BYTELEVEL;
+  const int64_t n_blk = ((int64_t)n + TSCAN - 1) / TSCAN;
+  const unsigned grid = (unsigned)(((uint64_t)n * 32 + DEC_THREADS - 1) / DEC_THREADS);
+  int rc;
+  if ((rc = ws.ctl.ensure(sizeof(DecodeCtl))) || (rc = ws.h_ctl.ensure(sizeof(DecodeCtl), false)) || (rc = ws.dec_count.ensure((size_t)n * 4 + 16)) ||
+      (rc = ws.dec_lexcl.ensure((size_t)n * 8 + 16)) || (rc = ws.dec_bsum.ensure((size_t)n_blk * 8 + 16)) || (rc = ws.dec_off.ensure(((size_t)n + 1) * 8)) ||
+      (lossy && ((rc = ws.dec_lcount.ensure((size_t)n * 4 + 16)) || (rc = ws.dec_lexcl2.ensure((size_t)n * 8 + 16)) ||
+                 (rc = ws.dec_bsum2.ensure((size_t)n_blk * 8 + 16)) || (rc = ws.dec_off2.ensure(((size_t)n + 1) * 8)))))
+    return rc;
+  DecodeCtl* ctl = ws.ctl.as<DecodeCtl>();
+  DecodeCtl* h = ws.h_ctl.as<DecodeCtl>();
+  CU(cudaMemsetAsync(ctl, 0, sizeof(DecodeCtl), st));
+  CU(cudaMemsetAsync(ws.dec_off.p, 0, 8, st));   // (text_off[0] of an empty batch)
+  rec(e, st, nullptr);
+  e->last_launches = 0;
+  if (n) {
+    decode_count_kernel<<<grid, DEC_THREADS, 0, st>>>(e->dec, R, skip, ws.dec_count.as<uint32_t>(), ctl);
+    tile_scan_block_kernel<<<(unsigned)n_blk, TSCAN, 0, st>>>(ws.dec_count.as<uint32_t>(), ws.dec_lexcl.as<unsigned long long>(), ws.dec_bsum.as<unsigned long long>(), n);
+    tile_scan_top_kernel<<<1, TSCAN, 0, st>>>(ws.dec_bsum.as<unsigned long long>(), n_blk, &ctl->total);
+    e->last_launches += 3;
+  }
+  rec(e, st, "decode_count");
+  CU(cudaMemcpyAsync(h, ctl, sizeof(DecodeCtl), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));   // the size of the text
+  if (h->err & DEC_ERR_ROWS) return fail(B2T_ERR_INVALID, "decode: row_ptr decreasing or a row outside [0, n_ids)");
+  if (h->err & DEC_ERR_ROW_SIZE) return fail(B2T_ERR_TOO_LARGE, "decode: the text of a row reaches %llu bytes; split the row", (unsigned long long)DEC_MAX_ROW_TEXT);
+  const uint64_t total = h->total;
+  if ((rc = ws.dec_text.ensure(total + 16))) return rc;
+  rec(e, st, "decode_size_read");   // (the host's read of the text size: not kernel time)
+  if (n)
+    decode_emit_kernel<<<grid, DEC_THREADS, 0, st>>>(e->dec, R, skip, ws.dec_count.as<uint32_t>(), ws.dec_lexcl.as<unsigned long long>(), ws.dec_bsum.as<unsigned long long>(),
+                                                     TSCAN, ws.dec_text.as<uint8_t>(), ws.dec_off.as<uint64_t>(), lossy ? ws.dec_lcount.as<uint32_t>() : nullptr, ctl);
+  e->last_launches++;
+  rec(e, st, "decode_emit");
+  *text = ws.dec_text.as<uint8_t>(); *text_off = ws.dec_off.as<uint64_t>(); *n_text = total;
+  if (!lossy || !n) { CU(cudaGetLastError()); return B2T_OK; }
+  CU(cudaMemcpyAsync(&h->bad, &ctl->bad, 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (!h->bad) return B2T_OK;   // valid UTF-8 throughout: the text is final
+  rec(e, st, "decode_flag_read");   // (the host's read of D2's flag: not kernel time)
+  // the scan of D2's lossy counts gives the rewritten text's exact size before its buffer is sized
+  tile_scan_block_kernel<<<(unsigned)n_blk, TSCAN, 0, st>>>(ws.dec_lcount.as<uint32_t>(), ws.dec_lexcl2.as<unsigned long long>(), ws.dec_bsum2.as<unsigned long long>(), n);
+  tile_scan_top_kernel<<<1, TSCAN, 0, st>>>(ws.dec_bsum2.as<unsigned long long>(), n_blk, &ctl->lossy);
+  rec(e, st, "decode_lossy_scan");
+  CU(cudaMemcpyAsync(&h->lossy, &ctl->lossy, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if ((rc = ws.dec_text2.ensure(h->lossy + 16))) return rc;
+  rec(e, st, "decode_lossy_read");   // (the host's read of the rewritten size: not kernel time)
+  decode_lossy_kernel<<<grid, DEC_THREADS, 0, st>>>(ws.dec_text.as<uint8_t>(), ws.dec_off.as<uint64_t>(), n, ws.dec_lcount.as<uint32_t>(), ws.dec_lexcl2.as<unsigned long long>(),
+                                                    ws.dec_bsum2.as<unsigned long long>(), TSCAN, ws.dec_text2.as<uint8_t>(), ws.dec_off2.as<uint64_t>());
+  e->last_launches += 3;
+  rec(e, st, "decode_lossy");
+  *text = ws.dec_text2.as<uint8_t>(); *text_off = ws.dec_off2.as<uint64_t>(); *n_text = h->lossy;
+  CU(cudaGetLastError());
+  return B2T_OK;
+}
+
+// argument checks shared by both decode entry points
+static int decode_args(const char* fn, b2t_engine* e, const void* ids, uint64_t n_ids, const uint64_t* row_ptr, uint32_t flags, b2t_result** out) {
+  if (!e || !out || !row_ptr || (!ids && n_ids)) return fail(B2T_ERR_INVALID, "%s: null argument", fn);
+  if (flags & ~(uint32_t)B2T_DECODE_SKIP_SPECIAL) return fail(B2T_ERR_INVALID, "%s: unknown flags 0x%x", fn, flags);
+  if (n_ids >= (1ull << 31)) return fail(B2T_ERR_TOO_LARGE, "%s: %llu ids exceed the per-call limit of 2^31 - 1; split the batch", fn, (unsigned long long)n_ids);
+  if (!e->dec_on) return fail(B2T_ERR_INVALID, "%s: the engine has no decoder (b2t_engine_set_decoder)", fn);
+  return B2T_OK;
+}
+
+extern "C" int b2t_decode_batch_device(b2t_engine* e, const uint32_t* d_ids, uint64_t n_ids, const uint64_t* d_row_ptr, const uint32_t* d_row_len,
+                                       uint32_t n_rows, uint32_t flags, void* stream, b2t_result** out) {
+  int rc = decode_args("b2t_decode_batch_device", e, d_ids, n_ids, d_row_ptr, flags, out);
+  if (rc) return rc;
+  std::lock_guard<std::mutex> lk(e->dev_mu);
+  CU(cudaSetDevice(e->device));
+  cudaStream_t st = stream ? (cudaStream_t)stream : e->own_stream;
+  Workspace& ws = e->dev_ws;
+  const uint8_t* text; const uint64_t* text_off; uint64_t n_text;
+  if ((rc = run_decode(e, ws, DecodeRows{d_ids, d_row_ptr, d_row_len, 0ull, n_ids, n_rows}, flags, st, &text, &text_off, &n_text))) return rc;
+  b2t_result* r = new b2t_result();
+  r->eng = e; r->on_device = 1; r->n_docs = n_rows; r->n_tokens = n_text;
+  r->view.text = text; r->view.text_off = text_off;
+  *out = r;
+  return B2T_OK;
+}
+
+// The host entry point: chunks of whole rows (ids spanning at most chunk_bytes / 4; a larger row is a chunk of its own) on
+// the slot set's workspaces in turn.  A chunk's text is copied into the pinned result on its slot's stream while the next
+// chunk is staged and decoded on the next slot.  That is the only overlap: a chunk's own kernels wait for the host's reads
+// of run_decode (the text size, and for ByteLevel the lossy flag), so the copies in, the kernels and the copies out of
+// one chunk do not overlap each other as they do in the encode pipeline.
+static int host_decode(b2t_engine* e, b2t_engine::SlotSet& ss, const uint32_t* ids, const uint64_t* row_ptr, const uint32_t* row_len, uint32_t n_rows,
+                       uint32_t flags, b2t_result** out) {
+  const uint64_t chunk_ids = std::max<uint64_t>(e->chunk_bytes / 4, 1);
+  auto row_end = [&](uint32_t r) { return row_len ? row_ptr[r] + row_len[r] : row_ptr[r + 1]; };
+  b2t_result* r = pool_get(e);
+  r->eng = e; r->on_device = 0; r->n_docs = n_rows; r->n_tokens = 0;
+  int rc;
+  uint64_t cap = 0, text_base = 0;
+  if ((rc = r->h_text_off.ensure(((size_t)n_rows + 1) * 8, false)) || (rc = r->h_text.ensure(16, false))) { pool_put(e, r); return rc; }
+  cap = r->h_text.cap;
+  uint64_t* toff = r->h_text_off.as<uint64_t>();
+  struct DecChunk { uint32_t r0, r1; uint64_t base; };
+  std::vector<DecChunk> chunks;
+  rc = B2T_OK;
+  for (uint32_t r0 = 0, ci = 0; r0 < n_rows && rc == B2T_OK; ++ci) {
+    const uint64_t lo = row_ptr[r0];
+    uint64_t hi = row_end(r0);
+    uint32_t r1 = r0 + 1;
+    while (r1 < n_rows && std::max(hi, row_end(r1)) - lo <= chunk_ids) hi = std::max(hi, row_end(r1++));
+    Workspace& ws = ss.slot[ci % NSLOT];
+    auto step = [&]() -> int {
+      int rc2;
+      if ((rc2 = slot_init(ws))) return rc2;
+      CU(cudaStreamSynchronize(ws.stream));   // (its previous chunk's copies have landed)
+      const uint32_t nr = r1 - r0;
+      if ((rc2 = ws.dec_ids.ensure((hi - lo) * 4 + 16)) || (rc2 = ws.dec_row_ptr.ensure(((size_t)nr + 1) * 8)) ||
+          (row_len && (rc2 = ws.dec_row_len.ensure((size_t)nr * 4 + 16))))
+        return rc2;
+      if (hi > lo) CU(cudaMemcpyAsync(ws.dec_ids.p, ids + lo, (hi - lo) * 4, cudaMemcpyHostToDevice, ws.stream));
+      CU(cudaMemcpyAsync(ws.dec_row_ptr.p, row_ptr + r0, ((size_t)nr + (row_len ? 0 : 1)) * 8, cudaMemcpyHostToDevice, ws.stream));
+      if (row_len) CU(cudaMemcpyAsync(ws.dec_row_len.p, row_len + r0, (size_t)nr * 4, cudaMemcpyHostToDevice, ws.stream));
+      const uint8_t* text; const uint64_t* text_off; uint64_t n_text;
+      if ((rc2 = run_decode(e, ws, DecodeRows{ws.dec_ids.as<uint32_t>(), ws.dec_row_ptr.as<uint64_t>(), row_len ? ws.dec_row_len.as<uint32_t>() : nullptr, lo, hi - lo, nr},
+                            flags, ws.stream, &text, &text_off, &n_text)))
+        return rc2;
+      if (text_base + n_text > cap) {
+        // earlier chunks may still be copying into the old buffer: let them land, then grow (contents are kept)
+        for (auto& s : ss.slot) if (s.stream) CU(cudaStreamSynchronize(s.stream));
+        if ((rc2 = r->h_text.ensure((text_base + n_text) * 2, true))) return rc2;
+        cap = r->h_text.cap;
+      }
+      if (n_text) CU(cudaMemcpyAsync(r->h_text.as<uint8_t>() + text_base, text, n_text, cudaMemcpyDeviceToHost, ws.stream));
+      CU(cudaMemcpyAsync(toff + r0, text_off, (size_t)nr * 8, cudaMemcpyDeviceToHost, ws.stream));
+      chunks.push_back({r0, r1, text_base});
+      text_base += n_text;
+      return B2T_OK;
+    };
+    rc = step();
+    r0 = r1;
+  }
+  for (auto& s : ss.slot) if (s.stream) cudaStreamSynchronize(s.stream);
+  if (rc) { pool_put(e, r); return rc; }
+  // chunk-relative offsets -> batch-relative
+  for (const DecChunk& c : chunks)
+    if (c.base) for (uint32_t k = c.r0; k < c.r1; ++k) toff[k] += c.base;
+  toff[n_rows] = text_base;
+  r->n_tokens = text_base;
+  r->view.text = r->h_text.as<uint8_t>(); r->view.text_off = toff;
+  *out = r;
+  return B2T_OK;
+}
+
+extern "C" int b2t_decode_batch(b2t_engine* e, const uint32_t* ids, uint64_t n_ids, const uint64_t* row_ptr, const uint32_t* row_len, uint32_t n_rows,
+                                uint32_t flags, b2t_result** out) {
+  int rc = decode_args("b2t_decode_batch", e, ids, n_ids, row_ptr, flags, out);
+  if (rc) return rc;
+  for (uint32_t r = 0; r < n_rows; ++r) {   // the kernels index the id buffer with these
+    if (r + 1 < n_rows && row_ptr[r + 1] < row_ptr[r]) return fail(B2T_ERR_INVALID, "b2t_decode_batch: row_ptr must be non-decreasing (row %u)", r);
+    const uint64_t end = row_len ? row_ptr[r] + row_len[r] : row_ptr[r + 1];
+    if (end < row_ptr[r] || end > n_ids) return fail(B2T_ERR_INVALID, "b2t_decode_batch: row %u lies outside [0, n_ids)", r);
+  }
+  std::unique_lock<std::mutex> prof(e->prof_mu, std::defer_lock);
+  SetLease lease(e);
+  if (e->profiling) prof.lock();
+  CU(cudaSetDevice(e->device));
+  return host_decode(e, *lease.ss, ids, row_ptr, row_len, n_rows, flags, out);
+}
+
 // ------------------------------------------------------------------------------------------------ results
 extern "C" uint64_t b2t_result_n_tokens(const b2t_result* r) { return r ? r->n_tokens : 0; }
 extern "C" uint32_t b2t_result_n_docs(const b2t_result* r) { return r ? r->n_docs : 0; }
@@ -1578,6 +1803,8 @@ extern "C" const uint32_t* b2t_result_dense_offsets(const b2t_result* r) { retur
 extern "C" const uint8_t* b2t_result_special_tokens_mask(const b2t_result* r) { return dense_view<uint8_t>(r, OUT_SPECIAL); }
 extern "C" const int8_t* b2t_result_sequence_ids(const b2t_result* r) { return dense_view<int8_t>(r, OUT_SEQ); }
 extern "C" const uint32_t* b2t_result_dense_word_ids(const b2t_result* r) { return dense_view<uint32_t>(r, OUT_WORD); }
+extern "C" const uint8_t* b2t_result_text(const b2t_result* r) { return r ? r->view.text : nullptr; }
+extern "C" const uint64_t* b2t_result_text_off(const b2t_result* r) { return r ? r->view.text_off : nullptr; }
 extern "C" void b2t_result_free(b2t_result* r) {
   if (!r) return;
   if (r->on_device || !r->eng) { delete r; return; }

@@ -1,6 +1,8 @@
 // host_tables.cu -- see host_tables.h
 #include "host_tables.h"
 
+#include "../../include/b2t.h"
+
 #include <string.h>
 #include <vector_types.h>
 
@@ -356,6 +358,91 @@ std::string build_host_tables(int model, int pretok, int ignore_merges, uint32_t
       out->edge_tbl[slot] = make_uint4((uint32_t)kv.first, kv.second, node_tok[kv.second], 0);
     }
   }
+  return "";
+}
+
+}  // namespace b2t
+
+namespace b2t {
+
+// decoders/wordpiece.rs:31-44 cleanup(): the replacements in order, each over the whole string
+static void wordpiece_cleanup(std::string& s) {
+  static const char* const from_to[][2] = {{" .", "."}, {" ?", "?"}, {" !", "!"}, {" ,", ","}, {" ' ", "'"}, {" n't", "n't"},
+                                           {" 'm", "'m"}, {" do not", " don't"}, {" 's", "'s"}, {" 've", "'ve"}, {" 're", "'re"}};
+  for (const auto& ft : from_to) {
+    const std::string a = ft[0], b = ft[1];
+    std::string r;
+    size_t i = 0;
+    for (size_t j; (j = s.find(a, i)) != std::string::npos; i = j + a.size()) r.append(s, i, j - i).append(b);
+    r.append(s, i, std::string::npos);
+    s.swap(r);
+  }
+}
+
+// byte_level.rs:156-171 per token: every char through the inverse byte map, or the token's own UTF-8 when a char is not in it
+static std::string bytelevel_image(const std::string& t, const int16_t* byte_of_cp, uint32_t n_cp) {
+  std::string r;
+  for (size_t i = 0; i < t.size();) {
+    const uint8_t b = (uint8_t)t[i];
+    const uint32_t n = b < 0x80 ? 1 : (b >> 5) == 6 ? 2 : (b >> 4) == 14 ? 3 : (b >> 3) == 30 ? 4 : 0;
+    if (n == 0 || i + n > t.size()) return t;
+    uint32_t cp = n == 1 ? b : b & (0x7Fu >> n);
+    for (uint32_t k = 1; k < n; ++k) cp = cp << 6 | ((uint8_t)t[i + k] & 63u);
+    if (cp >= n_cp || byte_of_cp[cp] < 0) return t;
+    r.push_back((char)byte_of_cp[cp]);
+    i += n;
+  }
+  return r;
+}
+
+std::string build_decoder_table(int kind, const char* prefix, bool cleanup, bool normalizer, uint32_t n_vocab, const uint8_t* vocab_bytes,
+                                const uint32_t* vocab_off, const uint32_t* vocab_ids, uint32_t n_added, const uint8_t* added_bytes,
+                                const uint32_t* added_off, const uint32_t* added_ids, const uint8_t* added_flags, DecoderHost* out) {
+  if (kind != B2T_DECODER_NONE && kind != B2T_DECODER_BYTELEVEL && kind != B2T_DECODER_WORDPIECE) return "decoder kind " + std::to_string(kind) + " is not supported on the device";
+  // id -> string: the model's, then the added vocabulary's over it
+  uint32_t n_ids = 0;
+  for (uint32_t i = 0; i < n_vocab; ++i) n_ids = std::max(n_ids, vocab_ids[i] + 1);
+  for (uint32_t i = 0; i < n_added; ++i) n_ids = std::max(n_ids, added_ids[i] + 1);
+  for (uint32_t i = 0; i < n_vocab; ++i) if (vocab_ids[i] >= DEC_MAX_IDS) return "vocabulary id " + std::to_string(vocab_ids[i]) + ": ids of 2^20 and above are not supported";
+  for (uint32_t i = 0; i < n_added; ++i) if (added_ids[i] >= DEC_MAX_IDS) return "added token id " + std::to_string(added_ids[i]) + ": ids of 2^20 and above are not supported";
+  std::vector<const uint8_t*> str(n_ids, nullptr);
+  std::vector<uint32_t> len(n_ids, 0);
+  for (uint32_t i = 0; i < n_vocab; ++i) { str[vocab_ids[i]] = vocab_bytes + vocab_off[i]; len[vocab_ids[i]] = vocab_off[i + 1] - vocab_off[i]; }
+  std::unordered_map<std::string, bool> special;
+  for (uint32_t i = 0; i < n_added; ++i) {
+    if (normalizer && (added_flags[i] & B2T_ADDED_NORMALIZED))
+      return "added tokens with normalized=true behind a normalizer: their decoded string is not settled (the normalized form or the content)";
+    str[added_ids[i]] = added_bytes + added_off[i]; len[added_ids[i]] = added_off[i + 1] - added_off[i];
+    if (added_flags[i] & B2T_ADDED_SPECIAL) special[std::string((const char*)added_bytes + added_off[i], added_off[i + 1] - added_off[i])] = true;
+  }
+  int16_t byte_of_cp[0x144];
+  std::fill(byte_of_cp, byte_of_cp + 0x144, (int16_t)-1);
+  uint32_t cp_of_byte[256];
+  bytes_char_table(cp_of_byte);
+  for (int b = 0; b < 256; ++b) byte_of_cp[cp_of_byte[b]] = (int16_t)b;
+  const std::string pre = prefix ? prefix : "";
+  out->ent.assign(n_ids, 0ull);
+  out->pool.clear();
+  for (uint32_t id = 0; id < n_ids; ++id) {
+    if (!str[id]) continue;
+    const std::string t((const char*)str[id], len[id]);
+    std::string first, rest;
+    if (kind == B2T_DECODER_BYTELEVEL) first = rest = bytelevel_image(t, byte_of_cp, 0x144);
+    else if (kind == B2T_DECODER_NONE) { first = t; rest = " " + t; }
+    else {   // wordpiece.rs:47-61: a later token loses the prefix or gains a space, then cleanup on the token alone
+      first = t;
+      rest = t.compare(0, pre.size(), pre) == 0 ? t.substr(pre.size()) : " " + t;
+      if (cleanup) { wordpiece_cleanup(first); wordpiece_cleanup(rest); }
+    }
+    if (first.size() > DEC_LEN_MASK || rest.size() > DEC_LEN_MASK) return "token " + std::to_string(id) + ": a decoded image over 16383 bytes is not supported";
+    if (out->pool.size() + first.size() + rest.size() >= (1ull << 32)) return "decoder images over 4 GiB are not supported";
+    const uint64_t off = out->pool.size();
+    out->pool.insert(out->pool.end(), first.begin(), first.end());
+    out->pool.insert(out->pool.end(), rest.begin(), rest.end());
+    const uint32_t meta = (uint32_t)first.size() | (uint32_t)rest.size() << DEC_LEN_BITS | DEC_EXISTS | (special.count(t) ? DEC_SKIP : 0u);
+    out->ent[id] = off | (uint64_t)meta << 32;
+  }
+  out->pool.resize(out->pool.size() + 16, 0);
   return "";
 }
 

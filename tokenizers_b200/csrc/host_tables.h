@@ -50,6 +50,17 @@ void space_counts(const uint8_t* s, uint32_t len, const uint8_t* cls, uint32_t* 
 // Per vocabulary id (ids above the largest are not in the table): space_counts' lead | trail << 16 of its string.
 std::vector<uint32_t> vocab_trim_counts(uint32_t n_vocab, const uint8_t* vocab_bytes, const uint32_t* vocab_off, const uint32_t* vocab_ids);
 
+// The decoder table (b2t_tables.h DEC_*): entry per id in [0, largest id], images back to back in pool.  kind: 0 none, 1
+// ByteLevel, 2 WordPiece.  The added vocabulary wins over the model's (added_vocabulary.rs simple_id_to_token); a special
+// added token's content marks every id with that string.  Returns "" on success, else the reason for B2T_ERR_UNSUPPORTED.
+struct DecoderHost {
+  std::vector<uint64_t> ent;
+  std::vector<uint8_t> pool;
+};
+std::string build_decoder_table(int kind, const char* prefix, bool cleanup, bool normalizer, uint32_t n_vocab, const uint8_t* vocab_bytes,
+                                const uint32_t* vocab_off, const uint32_t* vocab_ids, uint32_t n_added, const uint8_t* added_bytes,
+                                const uint32_t* added_off, const uint32_t* added_ids, const uint8_t* added_flags, DecoderHost* out);
+
 // Returns "" on success, else an error message; *vocab_err distinguishes B2T_ERR_VOCAB from B2T_ERR_UNSUPPORTED.
 std::string build_host_tables(int model, int pretok, int ignore_merges, uint32_t n_vocab, const uint8_t* vocab_bytes,
                               const uint32_t* vocab_off, const uint32_t* vocab_ids, uint32_t n_merges,

@@ -183,6 +183,48 @@ def parse_tokenizer_json(js):
     return cfg
 
 
+def decoder_spec(decoder, added_tokens):
+    """tokenizer.json's decoder and the added vocabulary (objects with content, id, special, normalized) -> (b2t_decoder_spec,
+    the arrays it points into), or (None, reason) for a decoder the device does not run"""
+    ty = None if decoder is None else decoder.get("type")
+    kinds = {None: _lib.DECODER_NONE, "ByteLevel": _lib.DECODER_BYTELEVEL, "WordPiece": _lib.DECODER_WORDPIECE}
+    if ty not in kinds:
+        return None, f"decoder {ty} is not supported on the device (ByteLevel, WordPiece and no decoder are)"
+    toks = [t for t in added_tokens if t.content]
+    tb, to = _pack([t.content for t in toks], np.uint32)
+    ti = np.asarray([t.id for t in toks], dtype=np.uint32)
+    tf = np.asarray([(_lib.ADDED_SPECIAL if t.special else 0) | (_lib.ADDED_NORMALIZED if t.normalized else 0) for t in toks], dtype=np.uint8)
+    sp = _lib.DecoderSpec()
+    sp.struct_size = ctypes.sizeof(_lib.DecoderSpec)
+    sp.kind = kinds[ty]
+    sp.prefix = decoder.get("prefix", "##").encode("utf-8") if ty == "WordPiece" else None
+    sp.cleanup = int(bool(decoder.get("cleanup", True))) if ty == "WordPiece" else 0
+    sp.n_added = len(toks)
+    sp.added_bytes, sp.added_off, sp.added_ids, sp.added_flags = tb.ctypes.data, to.ctypes.data, ti.ctypes.data, tf.ctypes.data
+    return sp, (tb, to, ti, tf)
+
+
+def engine_config(cfg, device=-1):
+    """parse_tokenizer_json's dict -> (b2t_config, the arrays it points into)"""
+    vocab = cfg["vocab"]
+    toks = list(vocab.keys())
+    vb, vo = _pack(toks, np.uint32)
+    vi = np.fromiter((vocab[t] for t in toks), dtype=np.uint32, count=len(toks))
+    mb, mo = _pack([s for ab in cfg["merges"] for s in ab], np.uint32)
+    c = _lib.Config()
+    c.struct_size = ctypes.sizeof(_lib.Config)
+    c.model, c.pretok = cfg["model"], cfg["pretok"]
+    c.add_prefix_space, c.ignore_merges = cfg["add_prefix_space"], cfg["ignore_merges"]
+    c.n_vocab, c.vocab_bytes, c.vocab_off, c.vocab_ids = len(toks), vb.ctypes.data, vo.ctypes.data, vi.ctypes.data
+    c.n_merges, c.merge_bytes, c.merge_off = len(cfg["merges"]), mb.ctypes.data, mo.ctypes.data
+    c.unk_token = cfg["unk"].encode("utf-8") if cfg["unk"] is not None else None
+    c.continuing_subword_prefix = cfg["prefix"].encode("utf-8")
+    c.max_input_chars_per_word = cfg["max_chars"]
+    c.device = device
+    c.bert_normalizer = cfg.get("normalizer", 0)
+    return c, (vb, vo, vi, mb, mo)
+
+
 NO_WORD = 0xFFFFFFFF  # word id of a token the post-processor added (the reference reports None)
 
 
@@ -497,6 +539,15 @@ def _read_result(tok, res, views, zero_copy=False):
         L.b2t_result_free(res)
 
 
+def _device_view(torch, ptr, count, dtype, device):
+    """a torch tensor over `count` elements of device memory the engine owns (no copy)"""
+    typestr = {torch.uint8: "|u1", torch.int32: "<i4", torch.int64: "<i8"}[dtype]
+
+    class _Mem:
+        __cuda_array_interface__ = {"shape": (count,), "typestr": typestr, "data": (ptr, False), "version": 2}
+    return torch.as_tensor(_Mem(), device=device)
+
+
 def _byte_span(data, a0, b0, o0, o1, byte_offsets):
     """the byte span in data of a token with offsets (o0, o1) in the document data[a0:b0]; char offsets count the
     document's UTF-8 lead bytes"""
@@ -534,23 +585,9 @@ class Tokenizer:
         return tbl
 
     def _create_engine(self, device):
-        cfg = self._cfg
         L = _lib.lib()
-        toks = list(self._vocab.keys())
-        vb, vo = _pack(toks, np.uint32)
-        vi = np.fromiter((self._vocab[t] for t in toks), dtype=np.uint32, count=len(toks))
-        mb, mo = _pack([s for ab in cfg["merges"] for s in ab], np.uint32)
-        c = _lib.Config()
-        c.struct_size = ctypes.sizeof(_lib.Config)
-        c.model, c.pretok = cfg["model"], cfg["pretok"]
-        c.add_prefix_space, c.ignore_merges = cfg["add_prefix_space"], cfg["ignore_merges"]
-        c.n_vocab, c.vocab_bytes, c.vocab_off, c.vocab_ids = len(toks), vb.ctypes.data, vo.ctypes.data, vi.ctypes.data
-        c.n_merges, c.merge_bytes, c.merge_off = len(cfg["merges"]), mb.ctypes.data, mo.ctypes.data
-        c.unk_token = cfg["unk"].encode("utf-8") if cfg["unk"] is not None else None
-        c.continuing_subword_prefix = cfg["prefix"].encode("utf-8")
-        c.max_input_chars_per_word = cfg["max_chars"]
-        c.device = device
-        c.bert_normalizer = cfg.get("normalizer", 0)
+        c, _keep = engine_config(self._cfg, device)
+        self._device = device
         h = ctypes.c_void_p()
         rc = L.b2t_engine_create(ctypes.byref(c), ctypes.byref(h))
         if rc == _lib.B2T_ERR_UNSUPPORTED:
@@ -560,6 +597,27 @@ class Tokenizer:
         self._register_added()
 
     def _register_added(self):
+        """Hand the added vocabulary to the engine: to the extraction (b2t_engine_set_added_tokens) and, with the id -> string
+        map it changes, to the decoder (b2t_engine_set_decoder)."""
+        self._register_added_tokens()
+        self._set_decoder()
+
+    def _set_decoder(self):
+        """b2t_engine_set_decoder; a refusal only makes the device decode entry points unavailable (its reason is kept
+        for them to raise), it never fails construction"""
+        self._decoder_refused = "the tokenizer has no engine"
+        if getattr(self, "_h", None) is None:
+            return
+        L = _lib.lib()
+        sp, keep = decoder_spec(self._decoder, [] if self._added is None else list(self._added.tokens.values()))
+        if sp is None:
+            L.b2t_engine_set_decoder(self._h, None)
+            self._decoder_refused = keep
+            return
+        rc = L.b2t_engine_set_decoder(self._h, ctypes.byref(sp))
+        self._decoder_refused = None if rc == _lib.B2T_OK else L.b2t_last_error().decode("utf-8", "replace")
+
+    def _register_added_tokens(self):
         """Hand the added vocabulary to the engine (b2t_engine_set_added_tokens): the extraction then runs on the device.
         Configurations the device path refuses (add_prefix_space) keep the host extraction of added.py in front of the engine."""
         self._dev_added = False
@@ -1170,6 +1228,103 @@ class Tokenizer:
 
     def decode_batch(self, sequences, skip_special_tokens=True):
         return [self.decode(s, skip_special_tokens) for s in sequences]
+
+    # ---- device decode (b2t_decode_batch*): decode() of every row, on the GPU
+    def _decode_ready(self):
+        if self._decoder_refused is not None:
+            raise UnsupportedConfig(f"device decode is not available: {self._decoder_refused}")
+
+    @staticmethod
+    def _u32_ids(ids):
+        """integer ids -> uint32, ValueError for ids outside [0, 2^32) (the reference's binding takes u32)"""
+        a = np.asarray(ids)
+        if a.size and a.dtype.kind not in "iu":
+            raise ValueError(f"ids must be integers, not {a.dtype}")
+        if a.size and (int(a.min()) < 0 or int(a.max()) >= 1 << 32):
+            raise ValueError("ids must lie in [0, 2^32)")
+        return np.ascontiguousarray(a, dtype=np.uint32)
+
+    def decode_batch_csr(self, ids, row_ptr, skip_special_tokens=True):
+        """Rows of the token CSR (row d = ids[row_ptr[d]:row_ptr[d + 1]], as encode_batch_csr returns them) -> (text uint8,
+        text_off uint64[n + 1]): row d's text is text[text_off[d]:text_off[d + 1]], exactly decode(row, skip_special_tokens)"""
+        self._decode_ready()
+        ids = self._u32_ids(ids).reshape(-1)
+        rp = np.ascontiguousarray(row_ptr, dtype=np.uint64)
+        if rp.size == 0:
+            raise ValueError("row_ptr holds n_rows + 1 offsets")
+        return self._decode_host(ids, rp, None, rp.size - 1, skip_special_tokens)
+
+    def _decode_host(self, ids, row_ptr, row_len, n_rows, skip):
+        L = _lib.lib()
+        res = ctypes.c_void_p()
+        _lib.check(L.b2t_decode_batch(self._h, ids.ctypes.data if ids.size else None, ids.size, row_ptr.ctypes.data,
+                                      None if row_len is None else row_len.ctypes.data, n_rows, _lib.DECODE_SKIP_SPECIAL if skip else 0,
+                                      ctypes.byref(res)))
+        (text, off), _ = _read_result(self, res, lambda L, res: (_view(L.b2t_result_text(res), L.b2t_result_n_tokens(res), np.uint8),
+                                                               _view(L.b2t_result_text_off(res), n_rows + 1, np.uint64)))
+        return text, off
+
+    def decode_batch_rows(self, ids, lengths=None, skip_special_tokens=True):
+        """[n, L] rows of ids (numpy or torch; a CUDA tensor on the engine's device is decoded where it lies) -> n strings,
+        decode(row[:lengths[i]], skip_special_tokens) each; lengths=None decodes whole rows, padding included."""
+        self._decode_ready()
+        torch = None
+        if type(ids).__module__.startswith("torch"):
+            import torch
+        if torch is not None and ids.is_cuda and ids.device.index == (self._device if self._device >= 0 else torch.cuda.current_device()):
+            text, off = self._decode_rows_device(torch, ids, lengths, skip_special_tokens)
+        else:
+            a = ids.cpu().numpy() if torch is not None else ids
+            a = self._u32_ids(a)
+            if a.ndim != 2:
+                raise ValueError("ids must be [n, L]")
+            n, w = a.shape
+            if lengths is None:
+                text, off = self._decode_host(a.reshape(-1), np.arange(n + 1, dtype=np.uint64) * np.uint64(w), None, n, skip_special_tokens)
+            else:
+                ln = self._row_lengths(lengths.cpu().numpy() if hasattr(lengths, "cpu") else lengths, n, w)
+                text, off = self._decode_host(a.reshape(-1), np.arange(n, dtype=np.uint64) * np.uint64(w), ln.astype(np.uint32), n, skip_special_tokens)
+        tb = text.tobytes()
+        o = off.tolist()
+        return [tb[o[i]:o[i + 1]].decode("utf-8") for i in range(len(o) - 1)]
+
+    @staticmethod
+    def _row_lengths(lengths, n, w):
+        ln = np.asarray(lengths).reshape(-1)
+        if ln.shape != (n,) or (n and (ln.dtype.kind not in "iu" or int(ln.min()) < 0 or int(ln.max()) > w)):
+            raise ValueError(f"lengths must be {n} integers in [0, {w}]")
+        return ln
+
+    def _decode_rows_device(self, torch, ids, lengths, skip):
+        """b2t_decode_batch_device on a CUDA tensor (int64 is narrowed on the device) -> host (text, text_off)"""
+        if ids.dim() != 2:
+            raise ValueError("ids must be [n, L]")
+        if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
+            raise ValueError(f"ids must be integers, not {ids.dtype}")
+        n, w = ids.shape
+        if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= 1 << 32):
+            raise ValueError("ids must lie in [0, 2^32)")
+        dev = ids.device
+        ids32 = ids.to(torch.int32).contiguous()    # (the bit pattern of ids in [2^31, 2^32): unknown ids either way)
+        if lengths is None:
+            rp, rl = torch.arange(n + 1, device=dev, dtype=torch.int64) * w, None
+        else:
+            ln = torch.as_tensor(lengths, device=dev).reshape(-1)
+            if ln.shape[0] != n or (n and (ln.dtype.is_floating_point or int(ln.min()) < 0 or int(ln.max()) > w)):
+                raise ValueError(f"lengths must be {n} integers in [0, {w}]")
+            rp, rl = torch.arange(n, device=dev, dtype=torch.int64) * w, ln.to(torch.int32).contiguous()
+        L = _lib.lib()
+        res = ctypes.c_void_p()
+        st = torch.cuda.current_stream(dev).cuda_stream
+        _lib.check(L.b2t_decode_batch_device(self._h, ids32.data_ptr() if ids32.numel() else None, ids32.numel(), rp.data_ptr(),
+                                             None if rl is None else rl.data_ptr(), n, _lib.DECODE_SKIP_SPECIAL if skip else 0, st, ctypes.byref(res)))
+        try:
+            nb = L.b2t_result_n_tokens(res)
+            off = _device_view(torch, L.b2t_result_text_off(res), n + 1, torch.int64, dev).cpu().numpy().view(np.uint64)
+            text = _device_view(torch, L.b2t_result_text(res), nb, torch.uint8, dev).cpu().numpy() if nb else np.zeros(0, np.uint8)
+        finally:
+            L.b2t_result_free(res)
+        return text, off
 
     def pre_tokenize_batch(self, docs):
         """PreTokenizer seam: per document the list of (start_byte, end_byte) of its splits of the text as given (the
