@@ -166,6 +166,9 @@ __device__ __forceinline__ void wc_make_key(const uint8_t* s_byte, int s, int le
   key.slot = a;
   key.fp = ((((unsigned long long)b << 32) | a) ^ ((unsigned long long)len << 56)) & B2T_WC_FP;
   if (key.fp == 0) key.fp = 1;
+#ifdef B2T_WC_TEST_FP_MASK   // the host build in tests/native only: fingerprints that collide on purpose, so a hit rests on the key compare
+  key.fp = (key.fp & B2T_WC_TEST_FP_MASK) ? (key.fp & B2T_WC_TEST_FP_MASK) : 1ull;
+#endif
 }
 
 // Memory-model note.  A slot is written once per batch (the table is zeroed, stream-ordered, before the kernel) and never
@@ -175,13 +178,25 @@ __device__ __forceinline__ void wc_make_key(const uint8_t* s_byte, int s, int le
 // ids are < 2^20; the two length words carry a marker bit), all accesses are strong (.relaxed.gpu, single-copy atomic
 // per 32-bit word), and a reader accepts a slot only if the words it uses are non-zero and the whole key matches.  A word
 // that is not yet visible reads as zero, which is a miss: the pre-token is merged, the result is the same.
+// (The host branches serve the host build of the kernels in tests/native: the PTX memory model treats a vector access as
+// one access per element, so per-word relaxed atomics are the same thing.)
 __device__ __forceinline__ uint4 ld_relaxed_v4(const uint4* p) {
   uint4 v;
+#ifdef __CUDA_ARCH__
   asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
+#else
+  v.x = __atomic_load_n(&p->x, __ATOMIC_RELAXED); v.y = __atomic_load_n(&p->y, __ATOMIC_RELAXED);
+  v.z = __atomic_load_n(&p->z, __ATOMIC_RELAXED); v.w = __atomic_load_n(&p->w, __ATOMIC_RELAXED);
+#endif
   return v;
 }
 __device__ __forceinline__ void st_relaxed_v4(uint4* p, uint4 v) {
+#ifdef __CUDA_ARCH__
   asm volatile("st.relaxed.gpu.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+#else
+  __atomic_store_n(&p->x, v.x, __ATOMIC_RELAXED); __atomic_store_n(&p->y, v.y, __ATOMIC_RELAXED);
+  __atomic_store_n(&p->z, v.z, __ATOMIC_RELAXED); __atomic_store_n(&p->w, v.w, __ATOMIC_RELAXED);
+#endif
 }
 constexpr uint32_t WC_LEN_MARK = 0x80000000u;   // bit 31 of the second length word: always set in a written slot
 
@@ -254,7 +269,11 @@ __device__ __forceinline__ void wc_publish(const ModelParams& P, const uint8_t* 
     if (tag == 0ull) tag = atomicCAS(tagp, 0ull, B2T_WC_BUSY | key.fp);
     if (tag == 0ull) {  // the slot is ours
       uint32_t* kw = reinterpret_cast<uint32_t*>(q);
+#ifdef __CUDA_ARCH__
       asm volatile("st.relaxed.gpu.global.v2.u32 [%0], {%1, %2};" ::"l"(kw + 2), "r"(~key.k[0]), "r"(~key.k[1]) : "memory");
+#else
+      __atomic_store_n(kw + 2, ~key.k[0], __ATOMIC_RELAXED); __atomic_store_n(kw + 3, ~key.k[1], __ATOMIC_RELAXED);
+#endif
       st_relaxed_v4(q + 1, make_uint4(~key.k[2], ~key.k[3], ~key.k[4], ~key.k[5]));
       st_relaxed_v4(q + 2, make_uint4((uint32_t)nt | (lens[0] << 8) | (lens[1] << 16) | (lens[2] << 24), lens[3] | (lens[4] << 8) | (lens[5] << 16) | WC_LEN_MARK, ~ids[0], ~ids[1]));
       st_relaxed_v4(q + 3, make_uint4(~ids[2], ~ids[3], ~ids[4], ~ids[5]));
